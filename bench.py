@@ -1,23 +1,32 @@
 #!/usr/bin/env python
-"""bench.py — questions/sec of the N2NMN module-network hot path on B200 (BASELINE.json metric).
+"""bench.py — questions/sec of the N2NMN module-network hot path on H100 (BASELINE.json metric).
 
 One step = one pass of the hot path over one batch of synthetic input (default workload: CLEVR
 gt-layout eval, 64 questions, 10x15x512 pool5 grid, T=20 layout tokens, expert-layout mix): host
-layout compile (C++) -> table upload -> text projection -> tcgen05 conv_image contraction with the
+layout compile (C++) -> table upload -> text projection -> wgmma conv_image contraction with the
 fused Find epilogue -> tree kernel -> scores [64,28] on device. Inputs come from a pool of distinct
 batches resident in HBM that is larger than L2, walked round-robin, so no step re-reads a cached
 batch.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config clevr|shapes|vqa514|vqa2050|stress]
+                    [--dump-outputs DIR]
     python bench.py --impl reference ...        # CPU arm (the oracle restatement of the reference)
 
-How the number is taken (VERDICT r1: a 20-step region is ~1 ms of host wake-up noise): the block of
-K steps is repeated R times back to back, R chosen from a calibration run so that one timed region
-lasts >= --min-seconds (0.5 s), each region bracketed by barrier + synchronize and timed with CUDA
-events; `--trials` (3) regions are taken and the MEDIAN is reported (`repeats`, `timed_region_s`,
-`trial_values` are in the line). Under torchrun every rank owns one GPU and its own shard of the
-questions (weak scaling, no data-path collective: questions are independent, SURVEY.md §8e);
-region time = max over ranks; rank 0 prints ONE JSON line.
+How the number is taken: after W warm-up steps, one timed region is exactly K steps back to back,
+bracketed by barrier + synchronize and timed with CUDA events; `--trials` (5) such regions are
+taken and the MEDIAN is reported (`timed_steps` = K, `timed_region_s`, `trial_values` are in the
+line). Each region starts in steady state: right before it, one untimed launch set per context
+(`primer_steps`) is submitted, and the K steps are submitted while the GPU still runs it and the
+pool's worker threads are still awake. The host then gets ahead of the GPU only by what it can
+compile during the primer, as in a continuous stream, so host scheduling counts in the region
+whenever it is slower than the GPU. Successive regions walk the resident batches round-robin.
+Under torchrun every rank owns one GPU and its
+own shard of the questions (weak scaling, no data-path collective: questions are independent,
+SURVEY.md §8e); region time = max over ranks; rank 0 prints ONE JSON line.
+
+--dump-outputs DIR writes what the last timed step returned to its caller: DIR/scores.npy (float32
+[B, C]) and DIR/valid.npy (float32 0/1 [B]). Inputs, weights and layouts are seeded, so two builds
+run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -37,10 +46,6 @@ if ROOT not in sys.path:
 
 TEXT_DIM = 300
 UNIT = 'questions/s'
-# mma.sync.m16n8k8.tf32 issues once per ~36 cycles per SM sub-partition on this part (measured:
-# tools/ubench/mma_tf32.cu, DESIGN.md §4): 4 x 2048 flop / 36 clk x 148 SMs x 1.965 GHz. The
-# ceiling of every mma.sync kernel here (the fp32-parity text / quad products run 3 passes).
-MMA_SYNC_TF32_TFLOPS = 4 * 2048 / 36.0 * 148 * 1.965e9 / 1e12
 
 # BASELINE.json configs made concrete (SURVEY.md §0 table, §8d). `clevr` is the configuration the
 # metric is quoted on; the others are reported beside it (`other_configs`) or with --config.
@@ -61,7 +66,7 @@ WORKLOADS = {
                    metric='stress_questions_per_sec',
                    title='synthetic stress, batch=128/GPU, 20x20x1024 features, %s layouts depth<=16, T=40'),
 }
-L2_BYTES = 126e6
+L2_BYTES = 50e6   # H100
 
 
 def parse_args():
@@ -74,8 +79,8 @@ def parse_args():
     ap.add_argument('--batch', type=int, default=0, help='questions per GPU per step (0 = the config\'s)')
     ap.add_argument('--layouts', default=None, choices=['expert', 'random', 'deep'],
                     help='CLEVR layout set (default expert)')
-    ap.add_argument('--min-seconds', type=float, default=0.5, help='length of one timed region')
-    ap.add_argument('--trials', type=int, default=3, help='timed regions; the median is reported')
+    ap.add_argument('--min-seconds', type=float, default=0.0, help='ignored (old command lines)')
+    ap.add_argument('--trials', type=int, default=5, help='timed regions; the median is reported')
     ap.add_argument('--cpu-seconds', type=float, default=10.0, help='cpu_baseline sample budget')
     ap.add_argument('--ref-seconds', type=float, default=0.0,
                     help='--impl reference: stop after this many seconds (0 = run all --steps)')
@@ -97,6 +102,8 @@ def parse_args():
                     help='contexts/streams/worker threads (0 = the library default)')
     ap.add_argument('--host-threads', type=int, default=0, help='ignored (old command lines)')
     ap.add_argument('--pool', type=int, default=0, help='ignored (old command lines)')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step as DIR/<name>.npy')
     return ap.parse_args()
 
 
@@ -108,22 +115,8 @@ def peaks():
         return dict(hbm_gbs=d['hbm_gbs'], bf16_tflops=d['bf16_tflops'],
                     bf16_sustained=d.get('bf16_tflops_sustained', d['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0,
-                source='fallback (B200_PROFILING.md)')
-
-
-def ncu_traffic(kernel, batches_per_launch):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed
-    `ncu --set full` capture of this same command (profiles/ncu_traffic.json); None when there
-    is no capture or it was taken with another number of batches per launch."""
-    p = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    if not os.path.exists(p):
-        return None
-    with open(p) as f:
-        d = json.load(f).get(kernel)
-    if not d or d.get('batches_per_launch', 8) != batches_per_launch:
-        return None
-    return d['dram_read_bytes'] + d['dram_write_bytes']
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=989.0,
+                source='NVIDIA H100 SXM data sheet (dense, 700 W), not measured')
 
 
 def workload_title(wl, layouts):
@@ -155,7 +148,7 @@ def make_tokens(asm, kind, n, T, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md): one
+    """nvidia-smi clocks / throttle reasons during the timed region: one
     `nvidia-smi -lms` process started right before the region and stopped right after it."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
@@ -491,6 +484,7 @@ class Bench:
         self.ex = self.pool.executors[0]
         self.nout = max(2 * self.K, 8)
         self.outs = [torch.empty((B, C), dtype=torch.float32, device=dev) for _ in range(self.nout)]
+        self.last_out = torch.empty((B, C), dtype=torch.float32, device=dev)
 
     def tok(self, i):
         return self.toks[i % len(self.toks)]
@@ -506,65 +500,71 @@ class Bench:
             self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX)
         return float(t.item())
 
-    def blocks(self, steps, toks=None):
-        """Pre-marshalled blocks of `steps` steps that together walk all P resident batches."""
-        P = self.P
-        nb = min(64, P // math.gcd(steps, P))
-        out = []
-        for b in range(nb):
-            idx = [(b * steps + j) % P for j in range(steps)]
-            tk = [(toks or self.toks)[i % len(toks or self.toks)] for i in idx]
-            out.append(self.pool.make_block([self.feats[i] for i in idx],
-                                            [self.wvs[i] for i in idx], tk,
-                                            [self.outs[(b * steps + j) % self.nout]
-                                             for j in range(steps)]))
-        return out
+    def block(self, start, steps, toks=None, last_out=None):
+        """Pre-marshalled block of `steps` steps over the resident batches start, start + 1, ...
+        (round-robin). `last_out`: output tensor of the last step (the others cycle through
+        self.outs, so two steps on different contexts may share a buffer)."""
+        idx = [(start + j) % self.P for j in range(steps)]
+        tk = [(toks or self.toks)[i % len(toks or self.toks)] for i in idx]
+        outs = [self.outs[j % self.nout] for j in range(steps)]
+        if last_out is not None:
+            outs[-1] = last_out
+        return self.pool.make_block([self.feats[i] for i in idx], [self.wvs[i] for i in idx], tk,
+                                    outs)
 
-    def region(self, blocks, repeats):
-        """`repeats` back-to-back repetitions of the step block, CUDA events on the current stream
-        (pool.begin()/end() order the pool's streams after e0 / before e1). Returns ms, max over
-        ranks, and the host time needed to enqueue."""
+    def region(self, blk, primer=None):
+        """One step block, CUDA events on the current stream (pool.begin()/end() order the pool's
+        streams after e0 / before e1). `primer`: untimed block submitted right before, so that the
+        timed steps start behind work the GPU is still running, with the workers awake. Returns
+        ms, max over ranks, and the host time needed to enqueue."""
         torch = self.torch
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         self.barrier()
+        if primer is not None:
+            self.pool.begin()
+            self.pool.submit_block(primer)
+            self.pool.end()
         e0.record()
         t0 = time.perf_counter()
         self.pool.begin()
-        for r in range(repeats):
-            self.pool.submit_block(blocks[r % len(blocks)])
+        self.pool.submit_block(blk)
         self.pool.end()
         e1.record()
         host_ms = (time.perf_counter() - t0) * 1e3
         self.barrier()
         return self.allmax(e0.elapsed_time(e1)), host_ms
 
-    def timed(self, steps, warmup, min_seconds, trials, toks=None):
-        """warm-up, calibration, then `trials` regions of >= min_seconds; median region reported."""
+    def timed(self, steps, warmup, trials, toks=None):
+        """warm-up, then `trials` regions of exactly `steps` steps each, every one behind a primer
+        of one launch set per context; median region reported."""
         if warmup > 0:
-            wb = self.blocks(warmup, toks)
-            self.region(wb[:1], 1)
-        blocks = self.blocks(steps, toks)
-        cal_ms, _ = self.region(blocks, max(1, len(blocks)))      # touches every resident batch
-        per_block = cal_ms / max(1, len(blocks))
-        # the first estimate includes the pipeline fill of a short region: refine it on ~15 % of
-        # the target length before fixing the number of repetitions
-        R1 = int(max(1, math.ceil(0.15 * min_seconds * 1e3 / max(per_block, 1e-6))))
-        cal_ms, _ = self.region(blocks, R1)
-        per_block = cal_ms / R1
-        R = int(max(1, math.ceil(min_seconds * 1e3 / max(per_block, 1e-6))))
+            self.region(self.block(0, warmup, toks))
+        pre = self.K * self.pool.max_group
+        blks = []
+        for i in range(trials):
+            start = warmup + i * (pre + steps)
+            blks.append((self.block(start, pre, toks),
+                         self.block(start + pre, steps, toks, last_out=self.last_out)))
         res = []
-        for _ in range(trials):
+        for primer, blk in blks:
             l0 = self.pool.launch_count()
-            ms, host_ms = self.region(blocks, R)
+            ms, host_ms = self.region(blk, primer)
             res.append((ms, host_ms, self.pool.launch_count() - l0))
+        self.last_block = blks[-1][1]
         res.sort()
         ms, host_ms, launches = res[len(res) // 2]
-        n_steps = R * steps
-        return {'ms_per_step': ms / n_steps, 'repeats': R, 'timed_steps': n_steps,
+        return {'ms_per_step': ms / steps, 'timed_steps': steps, 'primer_steps': pre,
                 'gpu_launches': int(launches),
-                'timed_region_s': ms * 1e-3, 'host_enqueue_ms_per_step': host_ms / n_steps,
-                'value': self.world * self.B * n_steps / (ms * 1e-3),
-                'trial_values': [self.world * self.B * n_steps / (r[0] * 1e-3) for r in res]}
+                'timed_region_s': ms * 1e-3, 'host_enqueue_ms_per_step': host_ms / steps,
+                'value': self.world * self.B * steps / (ms * 1e-3),
+                'trial_values': [self.world * self.B * steps / (r[0] * 1e-3) for r in res]}
+
+    def dump_outputs(self, d):
+        """The scores and validity the last step of the last timed region handed to its caller."""
+        os.makedirs(d, exist_ok=True)
+        blk = self.last_block
+        np.save(os.path.join(d, 'scores.npy'), self.last_out.cpu().numpy().astype(np.float32))
+        np.save(os.path.join(d, 'valid.npy'), blk['valid'][-1].astype(np.float32))
 
     def kernel_pass(self, n=30):
         """Per-launch CUDA events (library profiling mode) of the kernels AS LAUNCHED IN THE TIMED
@@ -610,7 +610,7 @@ class Bench:
             return b / d / 1e9, f / d / 1e12, b / d / 1e9 / pk['hbm_gbs'], f / d / 1e12 / tf32_peak
 
         out = {'kernel_us': kus}
-        proj = 'proj_umma_kernel'
+        proj = 'proj_wgmma_kernel'
         if proj in kus:
             gbs, tfs, hf, tf = frac(kus[proj], nb[1], nf[1])
             bound = 'hbm' if hf >= tf else 'tensor'
@@ -618,8 +618,6 @@ class Bench:
                 'kernel': proj, 'bound': bound, 'achieved': gbs if bound == 'hbm' else tfs,
                 'peak': pk['hbm_gbs'] if bound == 'hbm' else tf32_peak,
                 'unit': 'GB/s' if bound == 'hbm' else 'TFLOP/s', 'frac': max(hf, tf),
-                'traffic': (ncu_traffic(proj, self.pool.max_group) if self.wl is WORKLOADS['clevr']
-                            else None),
                 'hbm_frac': hf, 'tensor_frac_of_tf32_peak': tf, 'avg_launch_us': kus[proj],
                 'algorithmic_bytes_per_launch': nb[1], 'flops_per_launch': nf[1],
                 'peak_source': pk['source'] + '; TF32 peak taken as bf16 burst / 2',
@@ -639,17 +637,6 @@ class Bench:
                             'batches_per_launch': self.pool.max_group,
                             'share_of_step': kus[name] / total}
         try:    # derived figures; never allowed to cost the line
-            if self.wl is WORKLOADS['clevr'] and 'roofline_text' in out:
-                # the text kernel's governing limit is the mma.sync issue rate, not HBM: three
-                # error-compensated TF32 passes over [rows, 304] x [304, 256] (K, M padded)
-                r = out['roofline_text']
-                rows = nf[0] / (2.0 * TEXT_DIM * 250)
-                issued = 3 * 2.0 * rows * 304 * 256
-                tf = issued / (r['avg_launch_us'] * 1e-6) / 1e12
-                r['issue_rate'] = {'bound': 'mma.sync issue rate (fp32-parity 3xTF32)',
-                                   'issued_flops_per_launch': issued, 'achieved': tf,
-                                   'peak': MMA_SYNC_TF32_TFLOPS, 'unit': 'TFLOP/s',
-                                   'frac': tf / MMA_SYNC_TF32_TFLOPS, 'rows_per_launch': rows}
             if self.wl['family'] == 'clevr' and 'pool_kernel' in kus and self.pooled_roots > 0:
                 b = self.pooled_roots * self.wl['H'] * self.wl['W'] * self.wl['D'] * 4.0
                 gbs = b / (kus['pool_kernel'] * 1e-6) / 1e9
@@ -658,12 +645,11 @@ class Bench:
                     'peak': pk['hbm_gbs'], 'unit': 'GB/s', 'frac': gbs / pk['hbm_gbs'],
                     'avg_launch_us': kus['pool_kernel'], 'algorithmic_bytes_per_launch': b,
                     'pooled_roots_per_launch': self.pooled_roots,
-                    'traffic': ncu_traffic('pool_kernel', self.pool.max_group),
                     'batches_per_launch': self.pool.max_group,
                     'share_of_step': kus['pool_kernel'] / total,
                     'note': 'algorithmic = one H*W*D feature grid per pooled root (Describe 1, '
                             'SameProperty 2); grids the contraction has just read are partly '
-                            'served from L2 (traffic = DRAM bytes of the ncu capture)'}
+                            'served from L2'}
         except Exception as e:   # noqa: BLE001
             out['roofline_derived_error'] = repr(e)
         return out
@@ -747,7 +733,7 @@ class Bench:
     def close(self):
         self.pool = None
         self.ex = None
-        self.feats = self.wvs = self.outs = None
+        self.feats = self.wvs = self.outs = self.last_out = None
         self.torch.cuda.empty_cache()
 
 
@@ -779,15 +765,18 @@ def main():
     bn = Bench(torch, dist, args, wl, layouts, B, rank, world, dev, streams=args.streams or None,
                device_synth=(args.config not in ('clevr', 'shapes')))
     pool, ex, K = bn.pool, bn.ex, bn.K
+    num_sms = torch.cuda.get_device_properties(dev).multi_processor_count
     pk = peaks()
 
-    # ---- headline: device-resident inputs, median of `trials` regions of >= min_seconds
+    # ---- headline: device-resident inputs, median of `trials` regions of exactly --steps steps
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    head = bn.timed(args.steps, args.warmup, args.min_seconds, args.trials)
+    head = bn.timed(args.steps, args.warmup, args.trials)
     launches = head['gpu_launches']
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        bn.dump_outputs(args.dump_outputs)
 
     # ---- the other two layout sets of SURVEY.md §8(d) (CLEVR: random valid; deep), same pool
     other_sets = None
@@ -796,7 +785,7 @@ def main():
         for kind in ('random', 'deep'):
             otoks = [make_tokens(bn.asm, kind, B, wl['T'], seed=100 + 1000 * rank + i)
                      for i in range(8)]
-            r = bn.timed(min(args.steps, 100), 12, 0.25, 1, toks=otoks)
+            r = bn.timed(min(args.steps, 100), 12, 1, toks=otoks)
             other_sets[kind] = {'value': r['value'], 'unit': UNIT, 'steps': r['timed_steps'],
                                 'timed_region_s': r['timed_region_s'], 'nodes_per_batch': int(
                                     np.mean([int((t != bn.asm.EOS_idx).sum()) for t in otoks]))}
@@ -812,7 +801,7 @@ def main():
         Bs = B // world
         sb = Bench(torch, dist, args, wl, layouts, Bs, rank, world, dev,
                    streams=args.streams or None)
-        r = sb.timed(args.steps, args.warmup, 0.3, 1)
+        r = sb.timed(args.steps, args.warmup, 1)
         strong = {'value': r['value'], 'unit': UNIT, 'global_batch': B, 'batch_per_gpu': Bs,
                   'ms_per_step': r['ms_per_step'], 'timed_region_s': r['timed_region_s'],
                   'scaling': 'strong'}
@@ -821,7 +810,7 @@ def main():
     # ---- roofline of the dominant kernel + HBM fractions of the two latency kernels (rank 0)
     roof = bn.roofline(pk) if rank == 0 else {}
     if rank == 0 and 'roofline' in roof:
-        roof['roofline']['grid_ctas'] = pool.proj_ctas if pool.proj_ctas > 0 else 148
+        roof['roofline']['grid_ctas'] = pool.proj_ctas if pool.proj_ctas > 0 else num_sms
 
     # ---- config 3: policy-search train step (fwd + bwd + ONE NCCL all-reduce + clip + Adam),
     #      T=10 as in exp_clevr/train_clevr_rl_gt_layout.py; reported beside the eval headline
@@ -867,8 +856,7 @@ def main():
         troof = None
         if gflops and acc.get('feat_grad_kernel'):
             tfs = gflops / (acc['feat_grad_kernel'] * 1e-6) / 1e12
-            troof = {'kernel': 'wgrad_umma_kernel (dW = sum X^T B: tcgen05 kind::tf32, both operands '
-                               'MN-major via TMA)',
+            troof = {'kernel': 'wgrad_wgmma_kernel (dW = sum X^T B: wgmma TF32, operands staged transposed)',
                      'bound': 'tensor', 'achieved': tfs, 'peak': tf32_peak, 'unit': 'TFLOP/s',
                      'frac': tfs / tf32_peak, 'avg_launch_us': acc['feat_grad_kernel'],
                      'flops_per_launch': gflops,
@@ -894,7 +882,7 @@ def main():
 
     info = ex.last_step_info()
     pool_cfg = {'streams': K, 'host_threads': K, 'tree_cluster_ctas': pool.tree_cluster,
-                'proj_grid_ctas': pool.proj_ctas if pool.proj_ctas > 0 else 148}
+                'proj_grid_ctas': pool.proj_ctas if pool.proj_ctas > 0 else num_sms}
 
     # ---- the other BASELINE.json workloads at their real sizes (N=1 only): q/s, roofline, CPU port
     others = None
@@ -906,10 +894,10 @@ def main():
             try:
                 ob = Bench(torch, dist, args, w2, w2['layouts'], w2['B'], rank, world, dev,
                            streams=4, device_synth=(name != 'shapes'))
-                r = ob.timed(min(args.steps, 40), 8, 0.3, 1)
+                r = ob.timed(min(args.steps, 40), 8, 1)
                 entry = {'workload': workload_title(w2, w2['layouts']), 'value': r['value'],
                          'unit': UNIT, 'ms_per_step': r['ms_per_step'],
-                         'timed_region_s': r['timed_region_s'], 'repeats': r['repeats'],
+                         'timed_region_s': r['timed_region_s'],
                          'streams': ob.K, 'resident_batches': ob.P,
                          'cache': cache_note(ob)}
                 entry.update(ob.roofline(pk))
@@ -930,7 +918,7 @@ def main():
             'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': head['ms_per_step'],
             'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
             'dtype': 'tf32 (fp32 in/out, fp32 accumulate)', 'data': 'synthetic',
-            'repeats': head['repeats'], 'timed_steps': head['timed_steps'],
+            'timed_steps': head['timed_steps'], 'primer_steps': head['primer_steps'],
             'timed_region_s': head['timed_region_s'], 'trials': args.trials,
             'trial_values': head['trial_values'],
             'config': dict({'workload': workload_title(wl, layouts), 'global_batch': B * world,

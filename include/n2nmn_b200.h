@@ -1,5 +1,5 @@
 /*
- * n2nmn_b200 — C ABI of the B200-native N2NMN module-network hot path.
+ * n2nmn_b200 — C ABI of the H100-native N2NMN module-network hot path.
  *
  * The reference (ronghanghu/n2nmn) has no FFI of its own: its hot path is a chain of TensorFlow
  * graph calls made from Python. Each entry point below therefore names the reference *Python*
@@ -17,7 +17,7 @@
  *   - `stream` is a cudaStream_t passed as void* (0 = legacy default stream). All device work is
  *     enqueued on it; no call synchronises the device except where documented;
  *   - a ctx is not thread-safe: one ctx per GPU per host thread.
- *   - the library runs on sm_100a only and fails with N2NMN_ERR_DEVICE elsewhere. There is no
+ *   - the library runs on sm_90a only and fails with N2NMN_ERR_DEVICE elsewhere. There is no
  *     CPU fallback.
  */
 #ifndef N2NMN_B200_H_
@@ -39,7 +39,7 @@ enum n2nmn_status {
   N2NMN_OK = 0,
   N2NMN_ERR_ARG = -1,      /* bad argument / shape */
   N2NMN_ERR_CUDA = -2,     /* a CUDA call failed */
-  N2NMN_ERR_DEVICE = -3,   /* not an sm_100 device */
+  N2NMN_ERR_DEVICE = -3,   /* not an sm_90 device */
   N2NMN_ERR_STATE = -4,    /* weights / inputs not bound yet */
   N2NMN_ERR_CAPACITY = -5  /* batch / T / node count exceeds what the ctx was created for */
 };
@@ -71,7 +71,7 @@ enum n2nmn_op {
 };
 
 enum n2nmn_flags {
-  /* Compute the conv_image contraction with the fp32 CUDA-core kernel instead of the tcgen05
+  /* Compute the conv_image contraction with the fp32 CUDA-core kernel instead of the wgmma
    * TF32 tensor-core kernel. Verification aid (bit-compatible with nothing, but free of TF32
    * rounding); never the default. */
   N2NMN_FLAG_PROJ_FP32_SIMT = 1,
@@ -204,7 +204,7 @@ int n2nmn_forward_tokens(n2nmn_ctx* ctx, const float* feat_dev, const float* wor
  * word_vecs_dev[i] [T,N,text_dim], layout tokens tokens_host[i] [T,N] and writes scores_dev[i]
  * [N,num_choices] (validity_out may be NULL, or hold NULL entries). Results are those of
  * num_batches separate n2nmn_forward_tokens calls; the point is that a batch of 64 CLEVR
- * questions is ~4 us of tensor work, far too little to fill 148 SMs per launch, while the reference's
+ * questions is ~4 us of tensor work, far too little to fill the SMs per launch, while the reference's
  * eval loop (exp_clevr/eval_clevr.py:103-135) offers an endless stream of independent batches. */
 int n2nmn_forward_group(n2nmn_ctx* ctx, int num_batches, const float* const* feat_dev,
                         const float* const* word_vecs_dev, const int32_t* const* tokens_host,

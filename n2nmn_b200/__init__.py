@@ -1,4 +1,4 @@
-"""n2nmn_b200 — B200-native (sm_100a) implementation of the N2NMN module-network hot path.
+"""n2nmn_b200 — H100-native (sm_90a) implementation of the N2NMN module-network hot path.
 
 Public surface mirrors the reference: ``Assembler`` (models_*/nmn3_assembler.py), ``Modules``
 (models_*/nmn3_modules.py) and the layout executor of ``NMN3Model`` (models_*/nmn3_model.py).

@@ -121,11 +121,11 @@ SIGNATURES = {
 
 def load():
     global LIB_PATH
-    LIB_PATH = os.environ.get('N2NMN_LIB', LIB_PATH)   # experiment builds (tools/) only
+    LIB_PATH = os.environ.get('N2NMN_LIB', LIB_PATH)   # experiment builds (build_variant) only
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             'n2nmn_b200: %s is missing. Build it with `python -m n2nmn_b200.build` (needs nvcc, '
-            'sm_100a). There is no CPU fallback.' % LIB_PATH)
+            'sm_90a). There is no CPU fallback.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)     # AttributeError if the .so lacks a declared symbol

@@ -1,4 +1,4 @@
-"""Builds csrc/ into n2nmn_b200/lib/libn2nmn_b200.so with nvcc for sm_100a (in-tree, so the
+"""Builds csrc/ into n2nmn_b200/lib/libn2nmn_b200.so with nvcc for sm_90a (in-tree, so the
 binary travels to the GPU box with the repo snapshot). Also builds nothing else: the oracle is
 pure numpy."""
 from __future__ import annotations
@@ -13,7 +13,7 @@ LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'libn2nmn_b200.so')
 SOURCES = ['capi.cu', 'seq2seq.cu', 'schedule.cpp', 'pool.cpp', 'util.cpp']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
          '-Xcompiler', '-fPIC', '--shared', '-x', 'cu', '-Xptxas', '-v']
 
 
@@ -27,7 +27,7 @@ def needs_build():
 
 
 def build_variant(name, defines):
-    """Experiment builds (tools/): lib/libn2nmn_b200_<name>.so with extra -D flags; selected at
+    """Experiment builds: lib/libn2nmn_b200_<name>.so with extra -D flags; selected at
     run time with N2NMN_LIB=<path>. Never the default library."""
     os.makedirs(LIBDIR, exist_ok=True)
     out = os.path.join(LIBDIR, 'libn2nmn_b200_%s.so' % name)

@@ -148,7 +148,7 @@ constexpr int kBwdSlicesMax = 8;   // CTAs per splittable node (>= 19 of the 150
 // One CTA per NODE, one launch per depth level from the roots down (bwd_nodes lists the nodes by
 // depth): the gradient maps travel between the levels through c.gmap (a node's map feeds exactly
 // one parent, so its gradient row has one writer, and that writer ran in an earlier launch).
-// Round 1 walked a question's nodes inside one CTA: 64 CTAs on 148 SMs and the longest question
+// Round 1 walked a question's nodes inside one CTA: 64 CTAs on all the SMs and the longest question
 // (~10 dependent modules, each bound by its own reductions) set the time: 360 us.
 // Two instantiations: kTransform = true handles every op (the stencil backward of Transform keeps
 // ~170 registers busy: one CTA per SM) and runs the levels that contain Transform nodes; false
@@ -1084,7 +1084,7 @@ __global__ void train_scalars_kernel(const float* __restrict__ loss_sum,
 
 // tf.clip_by_norm per tensor, then Adam (TF: lr_t = lr*sqrt(1-b2^t)/(1-b1^t)). The new value also
 // goes straight to the variable's place in the context's weight buffer (plain or row-pitched copy,
-// prep.cuh RepackSeg): the re-pack pass after the step only has the K-major tcgen05 copies and the
+// prep.cuh RepackSeg): the re-pack pass after the step only has the K-major wgmma copies and the
 // Transform quadratic form left to do.
 __global__ void adam_clip_kernel(float* __restrict__ w, const float* __restrict__ g,
                                  float* __restrict__ m, float* __restrict__ v,

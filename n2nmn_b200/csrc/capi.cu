@@ -1,5 +1,5 @@
 // C ABI of the N2NMN module-network hot path (include/n2nmn_b200.h): context, weight packing,
-// input binding, schedule upload and kernel launches. sm_100a only; no CPU fallback.
+// input binding, schedule upload and kernel launches. sm_90a only; no CPU fallback.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -18,14 +18,14 @@
 #include "node_eval.cuh"
 #include "prep.cuh"
 #include "proj_simt.cuh"
-#include "proj_umma.cuh"
+#include "proj_wgmma.cuh"
 #include "schedule.hpp"
 #include "text_proj.cuh"
 #include "tree_kernel.cuh"
 #include "head_kernel.cuh"
 #include "backward.cuh"
-#include "wgrad_umma.cuh"
-#include "head_tail_umma.cuh"
+#include "head_tail_wgmma.cuh"
+#include "wgrad_wgmma.cuh"
 
 using namespace n2nmn;
 
@@ -146,15 +146,14 @@ struct n2nmn_ctx {
   float* dstencil = nullptr;
   float* gmap = nullptr;
   float* phi_buf = nullptr;
-  WgradMaps wg_maps;                       // tcgen05 weight-gradient kernel (wgrad_umma.cuh)
-  bool wg_ok = false;                      // shapes fit it (Mp == 256, Dk % 128 == 0, no re-pitch)
+  bool wg_ok = false;   // shapes fit wgrad_wgmma_kernel (Mp == 256, Dk % 128 == 0, no re-pitch)
   // many-class answer heads (C > 32): ê rows + score-row addresses of the roots of a launch, and
   // the fc_eltwise matrices with rows pitched to a multiple of 4 floats (cp.async alignment)
   float* ehat = nullptr;
   float** ehat_dst = nullptr;
   float* out_wp[NUM_OUT_SETS] = {};
   int Cp = 0;
-  // ... and its tcgen05 form (head_tail_umma.cuh): remainder plane of ê, W_outᵀ planes, maps
+  // ... and its wgmma form (head_tail_wgmma.cuh): remainder plane of ê, W_outᵀ planes, maps
   float* ehat_lo = nullptr;
   float* out_wt_hi[NUM_OUT_SETS] = {};
   float* out_wt_lo[NUM_OUT_SETS] = {};
@@ -277,26 +276,6 @@ int encode_2d(n2nmn_ctx* c, CUtensorMap* map, const float* base, uint64_t inner,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail(N2NMN_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult " + std::to_string(r));
-  return 0;
-}
-
-// [outer][rows][row_pitch] fp32 viewed as (32 elements, rows, blocks of 32 elements, outer) with box
-// (32, box_rows, box_blocks, 1): 128-byte swizzle with 32-byte atoms (the MN-major operand layout
-// of 4-byte tensor-core operands), rows beyond `rows` zero-filled.
-int encode_mn_blocks(n2nmn_ctx* c, CUtensorMap* map, const float* base, uint64_t cols, uint64_t rows,
-                     uint64_t outer, uint64_t row_pitch_elems, uint32_t box_rows,
-                     uint32_t box_blocks) {
-  cuuint64_t dims[4] = {32, rows, cols / 32, outer};
-  cuuint64_t strides[3] = {row_pitch_elems * sizeof(float), 32 * sizeof(float),
-                           rows * row_pitch_elems * sizeof(float)};
-  cuuint32_t box[4] = {32, box_rows, box_blocks, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = c->encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), dims,
-                         strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return fail(N2NMN_ERR_CUDA, "cuTensorMapEncodeTiled (4d) failed with CUresult " + std::to_string(r));
   return 0;
 }
 
@@ -467,9 +446,9 @@ int run_tables(n2nmn_ctx* c, n2nmn_sched* sc, float* const* scores_seg, float* a
     p.mslot = reinterpret_cast<const int32_t*>(d + o.mslot);
     p.num_images = (int)(S.mslot.size() / NUM_PROJ_SETS);
     p.mbuf = c->mbuf;
-    // persistent grid of CTA pairs (clusters of 2): pair i walks work items i, i + pairs, ...
+    // persistent grid: CTA i walks the tiles i, i + CTAs, ... (two tiles per work item)
     const int max_ctas = c->proj_max_ctas > 0 ? std::min(c->proj_max_ctas, c->num_sms) : c->num_sms;
-    const int pairs = std::max(1, std::min(p.num_work, max_ctas / 2));
+    const int ctas = std::max(1, std::min(2 * p.num_work, max_ctas));
     if (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) {
       const size_t smem = (size_t)(kSimtRows * kSimtKChunk + kSimtRows * c->Mp) * sizeof(float);
       proj_simt_kernel<<<2 * p.num_work, 256, smem, st>>>(p);
@@ -477,18 +456,17 @@ int run_tables(n2nmn_ctx* c, n2nmn_sched* sc, float* const* scores_seg, float* a
     } else {
       cudaLaunchConfig_t lc;
       std::memset(&lc, 0, sizeof(lc));
-      lc.gridDim = dim3((unsigned)(2 * pairs));
+      lc.gridDim = dim3((unsigned)ctas);
       lc.blockDim = dim3(kProjThreads);
-      lc.dynamicSmemBytes = proj_smem_bytes(S.train);
+      lc.dynamicSmemBytes = proj_smem_bytes();
       lc.stream = st;
       cudaLaunchAttribute attr[1];
       attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
       attr[0].val.programmaticStreamSerializationAllowed = 1;
       lc.attrs = attr;
       lc.numAttrs = pdl_ok() ? 1 : 0;
-      if (S.train) CUDA_TRY(cudaLaunchKernelEx(&lc, proj_umma_kernel<true>, c->tmaps, p));
-      else CUDA_TRY(cudaLaunchKernelEx(&lc, proj_umma_kernel<false>, c->tmaps, p));
-      prof_mark(c, "proj_umma_kernel", st);
+      CUDA_TRY(cudaLaunchKernelEx(&lc, proj_wgmma_kernel, c->tmaps, p));
+      prof_mark(c, "proj_wgmma_kernel", st);
     }
     ++c->launches;
   }
@@ -606,7 +584,7 @@ int run_tables(n2nmn_ctx* c, n2nmn_sched* sc, float* const* scores_seg, float* a
             tc.gridDim = dim3((unsigned)(c->Cpad / kHtN), (unsigned)((r1 - r0 + kHtM - 1) / kHtM));
             tc.blockDim = dim3(kHtThreads);
             tc.dynamicSmemBytes = kHtSmemBytes;
-            CUDA_TRY(cudaLaunchKernelEx(&tc, head_tail_umma_kernel, c->ht_maps[os], c->md.out_b[os],
+            CUDA_TRY(cudaLaunchKernelEx(&tc, head_tail_wgmma_kernel, c->ht_maps[os], c->md.out_b[os],
                                         (float* const*)c->ehat_dst, r0, r1 - r0,
                                         (int)c->cfg.num_choices, (int)c->cfg.map_dim));
             ++c->launches;
@@ -668,8 +646,8 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
   CUDA_TRY(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10)
-    return fail(N2NMN_ERR_DEVICE, std::string("n2nmn_b200 needs an sm_100 GPU, found sm_") +
+  if (prop.major != 9)
+    return fail(N2NMN_ERR_DEVICE, std::string("n2nmn_b200 needs an sm_90 GPU, found sm_") +
                                       std::to_string(prop.major) + std::to_string(prop.minor));
   n2nmn_ctx* c = new n2nmn_ctx();
   c->cfg = *cfg;
@@ -798,7 +776,7 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
           if (int rc = encode_2d(c, &hm.b_hi, c->out_wt_hi[os], c->Mp, c->Cpad, c->Mp, kHtK, kHtN)) return rc;
           if (int rc = encode_2d(c, &hm.b_lo, c->out_wt_lo[os], c->Mp, c->Cpad, c->Mp, kHtK, kHtN)) return rc;
         }
-    CUDA_TRY(cudaFuncSetAttribute(head_tail_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CUDA_TRY(cudaFuncSetAttribute(head_tail_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)kHtSmemBytes));
     CUDA_TRY(cudaFuncSetAttribute(head_tail_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)mma_smem_bytes(2)));
@@ -875,11 +853,8 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
                                 c->node_smem_bytes));
   CUDA_TRY(cudaFuncSetAttribute(wave_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 c->node_smem_bytes));
-  CUDA_TRY(cudaFuncSetAttribute(proj_umma_kernel<true>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, proj_smem_bytes(true)));
-  CUDA_TRY(cudaFuncSetAttribute(proj_umma_kernel<false>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                proj_smem_bytes(false)));
+  CUDA_TRY(cudaFuncSetAttribute(proj_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                proj_smem_bytes()));
   CUDA_TRY(cudaFuncSetAttribute(
       proj_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
       (int)((kSimtRows * kSimtKChunk + kSimtRows * c->Mp) * sizeof(float))));
@@ -1360,7 +1335,7 @@ int forward_host_impl(n2nmn_ctx* c, int nb, const void* const* feat_host,
     const size_t cnt = fbytes / sizeof(float);
     for (int i = 0; i < nb; ++i) {
       const size_t n8 = (cnt + 7) / 8;
-      widen_f16_kernel<<<(unsigned)std::min<size_t>((n8 + 255) / 256, 148 * 8), 256, 0, st>>>(
+      widen_f16_kernel<<<(unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)c->num_sms * 8), 256, 0, st>>>(
           reinterpret_cast<const uint4*>(c->e2e_feat_f16 + i * fcap16),
           reinterpret_cast<float4*>(c->e2e_feat + i * fcap), n8);
       ++c->launches;
@@ -1529,13 +1504,9 @@ int n2nmn_train_backward(n2nmn_ctx* c, const float* feat_dev, const float* wv_de
     CUDA_TRY(cudaMalloc(&c->gmap, (size_t)c->arena_slots * ((c->HW + 3) & ~3) * sizeof(float)));
     CUDA_TRY(cudaMalloc(&c->phi_buf, (size_t)NB * 2 * c->Mp * sizeof(float)));
     c->wg_ok = c->Mp == kWgN && c->Dk % kWgM == 0 && !c->feat_aug;
-    if (c->wg_ok) {
-      if (int rc = encode_mn_blocks(c, &c->wg_maps.b, c->dmap, c->Mp, c->HW, c->dmap_entries, c->Mp,
-                                    kWgP, kWgN / 32))
-        return rc;
-      CUDA_TRY(cudaFuncSetAttribute(wgrad_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    if (c->wg_ok)
+      CUDA_TRY(cudaFuncSetAttribute(wgrad_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)kWgSmemBytes));
-    }
     const BwdSmem L = bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, c->cfg.kernel_size, C);
     const int bwd_smem = (int)(L.total * sizeof(float));
     CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
@@ -1620,9 +1591,9 @@ int n2nmn_train_backward(n2nmn_ctx* c, const float* feat_dev, const float* wv_de
     const int n_tr = S.bwd_ptr[2 * dd + 1] - S.bwd_ptr[2 * dd];
     const bool has_tr = n_tr > 0;
     // CTAs per splittable node: as many as keep the level's heavy CTAs within one wave of the
-    // SMs (148 at one CTA per SM with Transform nodes, 296 without)
-    const int slices = has_tr ? std::max(3, std::min(kBwdSlicesMax, 148 / n_tr))
-                              : std::max(2, std::min(6, 296 / cnt));
+    // SMs (one CTA per SM with Transform nodes, two without)
+    const int slices = has_tr ? std::max(3, std::min(kBwdSlicesMax, c->num_sms / n_tr))
+                              : std::max(2, std::min(6, 2 * c->num_sms / cnt));
     cudaLaunchConfig_t bl;
     std::memset(&bl, 0, sizeof(bl));
     bl.gridDim = dim3(cnt, slices);
@@ -1690,31 +1661,28 @@ int n2nmn_train_backward(n2nmn_ctx* c, const float* feat_dev, const float* wv_de
               (ne + per - 1) / per);
       feat_grad_kernel<<<g2, 256, 0, st>>>(c->md, c->dmap, d_ent, ne, per, gflat_dev, c->go);
     } else if (c->wg_ok && !std::getenv("N2NMN_WGRAD_MMA_SYNC")) {
-      // tcgen05, both operands MN-major straight from the feature grid and the B maps
-      if (int rc = encode_mn_blocks(c, &c->wg_maps.x, c->md.feat, c->Dk, c->HW, N, c->md.feat_pitch,
-                                    kWgP, kWgM / 32))
-        return rc;
+      // wgmma, both operands staged transposed (K-major) from the feature grid and the B maps
       const int slabs = c->Dk / kWgM;
-      const int chunks = std::max(1, std::min(ne, 148 / slabs));
+      const int chunks = std::max(1, std::min(ne, c->num_sms / slabs));
       WgradParams wp;
-      wp.entries = d_ent;
+      wp.feat = c->md.feat; wp.dmap = c->dmap; wp.entries = d_ent;
       wp.order = reinterpret_cast<const int32_t*>(d + o.entry_order);
       wp.num_entries = ne; wp.per_cta = (ne + chunks - 1) / chunks;
-      wp.HW = c->HW; wp.Dk = c->Dk; wp.M = c->cfg.map_dim; wp.gflat = gflat_dev; wp.go = c->go;
+      wp.HW = c->HW; wp.Dk = c->Dk; wp.M = c->cfg.map_dim; wp.Mp = c->Mp;
+      wp.pitch = c->md.feat_pitch; wp.gflat = gflat_dev; wp.go = c->go;
       dim3 gw(slabs, (ne + wp.per_cta - 1) / wp.per_cta);
-      wgrad_umma_kernel<<<gw, kWgThreads, kWgSmemBytes, st>>>(c->wg_maps, wp);
+      wgrad_wgmma_kernel<<<gw, kWgThreads, kWgSmemBytes, st>>>(wp);
       prof_mark(c, "feat_grad_kernel", st);
       bmap_colsum_kernel<<<ne, 1024, 0, st>>>(c->dmap, d_ent, c->HW, c->cfg.map_dim, c->Mp, gflat_dev,
                                              c->go);
-      ++c->launches;
-      ++c->launches;
+      c->launches += 2;
       prof_mark(c, "bias_grad_kernel", st);
       CUDA_TRY(cudaGetLastError());
       return 0;
     } else {
-      // two CTAs per SM (106 KB of ring each): ~296 CTAs over (Dk/128) x (M/64) tiles
+      // two CTAs per SM (106 KB of ring each): ~2 x SMs CTAs over (Dk/128) x (M/64) tiles
       const int tiles = ((c->Dk + kXtbM - 1) / kXtbM) * ((c->cfg.map_dim + kXtbN - 1) / kXtbN);
-      const int chunks = std::max(1, std::min(ne, (2 * 148 + tiles - 1) / tiles));
+      const int chunks = std::max(1, std::min(ne, (2 * c->num_sms + tiles - 1) / tiles));
       const int per = (ne + chunks - 1) / chunks;
       FeatGradSrc fs{c->md, c->dmap, d_ent, ne, gflat_dev, c->go};
       dim3 g2((c->Dk + kXtbM - 1) / kXtbM, (c->cfg.map_dim + kXtbN - 1) / kXtbN,

@@ -1,4 +1,4 @@
-// Shared device-side types and helpers for the N2NMN module-network kernels (sm_100a).
+// Shared device-side types and helpers for the N2NMN module-network kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -111,11 +111,10 @@ __host__ __device__ inline int quad_pitch(int ksize) { return (quad_rows(ksize) 
 // Host-compiled launch tables (built by schedule.cpp, consumed by the kernels).
 struct TextGroup { int32_t set, start, count, pad; };   // <= kTextRowsPerCta rows of one text set
 constexpr int kTextRowsPerCta = 64;
-// One work item of the contraction kernel = a PAIR of 128-row tiles of the same weight set, one per
-// CTA of a cta_group::2 pair (the tiles share nothing but the weight matrix, so they may come from
-// different images, passes or segments). row0 = first row inside the segment's [N*HW] row axis;
-// pass = which block of <= 8 Find consumers the fused epilogue serves, or -1 for a filler tile
-// (odd tile count: the MMA runs, nothing is written).
+// One work item of the contraction kernel = a PAIR of 128-row tiles of the same weight set (the
+// tiles share nothing but the weight matrix, so they may come from different images, passes or
+// segments). row0 = first row inside the segment's [N*HW] row axis; pass = which block of <= 8
+// Find consumers the fused epilogue serves, or -1 for a filler tile (odd tile count: skipped).
 struct ProjWork { int32_t row0[2], seg[2], pass[2], set, pad; };
 // One CTA of the answer-head kernel (head_kernel.cuh): `count` <= kHeadNodesMax root nodes of
 // the same type (Describe or SameProperty), listed in head_list[first .. first+count).

@@ -99,8 +99,7 @@ __host__ __device__ inline HeadSmem head_smem_layout(int nn, int pitch, int Mp) 
 // Precision: the pooled features enter as a TF32 hi + lo pair (split once when they are staged, so
 // they lose nothing), the weights are rounded to TF32 (cvt.rna) as they are loaded — the same
 // operand rounding the stored maps this replaces had on BOTH operands. (Splitting the weights as
-// well made the loop issue-bound: cvt.rna.tf32 is a multi-instruction sequence on sm_100, measured
-// 33 K cycles per product instead of ~12 K.)
+// well made the loop issue-bound: cvt.rna.tf32 is a multi-instruction sequence.)
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
   const float r = x - __uint_as_float(hi);

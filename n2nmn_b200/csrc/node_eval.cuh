@@ -37,7 +37,7 @@ struct NodeCtx {
   // root r (its position in the head list) in ehat[r][Mp] and the address of its score row in
   // ehat_dst[r]; head_tail_gemm_kernel does the fc_eltwise product as one GEMM (nullptr otherwise)
   float* ehat;
-  float* ehat_lo;      // ê - trunc_tf32(ê) for the tcgen05 tail (head_tail_umma.cuh), or nullptr
+  float* ehat_lo;      // ê - trunc_tf32(ê) for the wgmma tail (head_tail_wgmma.cuh), or nullptr
   float** ehat_dst;
 };
 

@@ -3,11 +3,11 @@
 //
 // A step's host work (layout compile ~10 us, table upload, three launches) is about as long as its
 // GPU work at batch 64, and ONE batch of 64 questions is ~4 us of tensor work — far too little to
-// fill 148 SMs per launch. So every context (= stream) has its own worker thread with a job queue;
+// fill the SMs per launch. So every context (= stream) has its own worker thread with a job queue;
 // n2nmn_pool_submit only copies the token matrix into a job and returns, and a worker takes up to
 // n2nmn_max_group(ctx) queued jobs of identical shape at a time and evaluates them with ONE set of
-// launches (n2nmn_forward_group): the contraction kernel then walks several tiles per CTA pair and
-// its epilogues overlap the next tile's MMAs. A worker never waits for more jobs: with one job
+// launches (n2nmn_forward_group): the contraction kernel then walks several tiles per CTA and
+// its TMA ring fills for the next tile while an epilogue runs. A worker never waits for more jobs: with one job
 // queued it runs one. There is no reference counterpart: the reference's executor is a Python loop
 // around session.run (exp_clevr/eval_clevr.py:96-133), one batch at a time.
 //

@@ -8,7 +8,7 @@
 namespace n2nmn {
 
 // W [K][M] (TF layout, models_clevr/nmn3_modules.py:101 'conv_image/weights') ->
-// Wt [Mp][Kp] K-major with zero padding: the B operand layout of the tcgen05 contraction.
+// Wt [Mp][Kp] K-major with zero padding: the B operand layout of the wgmma contraction.
 __global__ void transpose_pad_kernel(const float* __restrict__ W, int K, int M,
                                      float* __restrict__ Wt, int Kp, int Mp) {
   __shared__ float tile[32][33];
@@ -75,7 +75,7 @@ __global__ void repack_all_kernel(const float* __restrict__ wflat, const RepackS
     }
   }
 }
-// The K-major padded copies of the conv_image / fc_att weights (tcgen05 B operand) and their padded
+// The K-major padded copies of the conv_image / fc_att weights (wgmma B operand) and their padded
 // biases, every projection set in one launch: grid = (Kp/32, Mp/32, sets), block (32, 8).
 struct ProjRepack {
   int w_off[NUM_PROJ_SETS], b_off[NUM_PROJ_SETS];   // offsets in the flat buffer (-1: set not owned)

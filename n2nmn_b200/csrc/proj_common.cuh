@@ -1,5 +1,5 @@
 // Work description shared by the two implementations of the conv_image contraction
-// (tcgen05 TF32: proj_umma.cuh; fp32 CUDA cores: proj_simt.cuh).
+// (wgmma TF32: proj_wgmma.cuh; fp32 CUDA cores: proj_simt.cuh).
 //
 // The contraction  m[r, :] = X[r, :] · W_img + b_img  runs over the flattened (image, pixel) row
 // axis r = b*HW + p of the feature grid (models_clevr/nmn3_modules.py:101 through

@@ -25,8 +25,7 @@
 // programmatic dependent launch: each kernel requests what does not depend on its predecessor
 // (weights, tables) before griddepcontrol.wait.
 // At N = 64 an LSTM launch costs the issue time of its mma.sync instructions (three passes for fp32
-// parity; DESIGN.md §4c): the next step for this row is a persistent tcgen05 kernel with the
-// weights resident in shared memory.
+// parity; DESIGN.md §4c).
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -485,6 +484,7 @@ struct S2SVar {
 
 struct n2nmn_seq2seq {
   n2nmn_seq2seq_config cfg;
+  int num_sms = 0;
   std::vector<S2SVar> vars;
   bool dirty = true, tables_set = false;
   const float* sample_u = nullptr;   // [T_decoder][N] uniforms of the following forward calls
@@ -523,7 +523,9 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
 }
 
 // 32-row tiles while 64-row tiles would leave SMs without a CTA
-bool narrow_tiles(int col_blocks, int R) { return R > 16 && col_blocks * ((R + 63) / 64) < 148; }
+bool narrow_tiles(int col_blocks, int R, int num_sms) {
+  return R > 16 && col_blocks * ((R + 63) / 64) < num_sms;
+}
 
 int launch_gemm(n2nmn_seq2seq* s, cudaStream_t st, const float* A, int lda, int R, int K,
                 const float* B, int ldb, int C, const float* bias, float* out, int ldo,
@@ -534,7 +536,7 @@ int launch_gemm(n2nmn_seq2seq* s, cudaStream_t st, const float* A, int lda, int 
   const int cb = (C + kMmaCols - 1) / kMmaCols;
   const bool exact = !(s->cfg.flags & N2NMN_SEQ2SEQ_FLAG_TF32) || force_exact;
   const dim3 gn(cb, (R + 31) / 32), gw(cb, (R + 63) / 64), blk(kMmaThreads);
-  if (narrow_tiles(cb, R)) {
+  if (narrow_tiles(cb, R, s->num_sms)) {
     if (exact) S2S_TRY(launch_pdl(s2s_gemm_kernel<2, true>, gn, blk, mma_smem_bytes(2), st, op, bias, out, ldo));
     else S2S_TRY(launch_pdl(s2s_gemm_kernel<2, false>, gn, blk, mma_smem_bytes(2), st, op, bias, out, ldo));
   } else {
@@ -559,7 +561,7 @@ int prepare(n2nmn_seq2seq* s, cudaStream_t st) {
   for (int side = 0; side < 2; ++side) {
     for (int l = 0; l < g.num_layers; ++l) {
       const int in = l == 0 ? (side == 0 ? g.embed_dim_txt : g.embed_dim_nmn) : L;
-      regroup_gates_kernel<<<148, 256, 0, st>>>(s->v(cell_prefix(side, l) + "weights"),
+      regroup_gates_kernel<<<s->num_sms, 256, 0, st>>>(s->v(cell_prefix(side, l) + "weights"),
                                                 s->w_cell[side][l], in + L, L);
       regroup_gates_kernel<<<8, 256, 0, st>>>(s->v(cell_prefix(side, l) + "biases"),
                                               s->b_cell[side][l], 1, L);
@@ -608,11 +610,12 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
   S2S_TRY(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   S2S_TRY(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10)
-    return fail_with(N2NMN_ERR_DEVICE, std::string("n2nmn_b200 needs an sm_100 GPU, found sm_") +
+  if (prop.major != 9)
+    return fail_with(N2NMN_ERR_DEVICE, std::string("n2nmn_b200 needs an sm_90 GPU, found sm_") +
                                            std::to_string(prop.major) + std::to_string(prop.minor));
   auto* s = new n2nmn_seq2seq;
   s->cfg = *cfg;
+  s->num_sms = prop.multiProcessorCount;
   const int C = 4 * L, N = cfg->max_batch, Vt = cfg->num_vocab_txt, Vn = cfg->num_vocab_nmn;
   const int Et = cfg->embed_dim_txt, En = cfg->embed_dim_nmn;
   auto add = [&](const std::string& name, std::vector<int64_t> shape) {
@@ -769,7 +772,7 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
   }
   init_state_kernel<<<(N + 127) / 128, 128, 0, st>>>(s->X, s->cur_tok, neg_entropy_dev, N, T_dec, Vn);
   ++s->launches;
-  const bool narrow = narrow_tiles(C / kMmaCols, N);
+  const bool narrow = narrow_tiles(C / kMmaCols, N, s->num_sms);
   const dim3 grid(C / kMmaCols, narrow ? (N + 31) / 32 : (N + 63) / 64);
   int cur = 0;   // h[l][cur] holds every layer's h_{t-1}
   bool ok = true;

@@ -8,7 +8,7 @@ Reference counterparts
   * util/clevr_train/data_reader.py:11-143  -> ClevrBatchLoader / DataReader (imdb .npy = pickled
     list of dicts, one feature .npy [1,H,W,D] per image, `prune_filter_module`, prefetch queue)
 
-B200-first differences (behaviour of the produced batches is the reference's, checked against
+H100-first differences (behaviour of the produced batches is the reference's, checked against
 fixtures made by running the reference files, tests/golden/make_golden_data.py):
   * feature grids are read straight into PINNED host buffers from a small ring, so a batch can be
     handed to ExecutorPool.submit_host (async H2D on the slot's stream) without a staging copy —

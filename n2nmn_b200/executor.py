@@ -291,7 +291,7 @@ class ExecutorPool:
     dynamic batching of the queued work.
 
     A batch of 64 questions is a short chain of small kernels (~4 us of tensor work) that cannot
-    fill 148 SMs on its own; successive batches are independent (eval). submit() only queues the
+    fill the SMs on its own; successive batches are independent (eval). submit() only queues the
     batch; each context's C++ worker thread (csrc/pool.cpp) takes up to `max_group` queued batches
     at a time and runs them with ONE set of launches (n2nmn_forward_group), so the contraction
     kernel's CTA pairs walk several tiles each and the kernels of different contexts overlap on

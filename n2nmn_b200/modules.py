@@ -48,7 +48,7 @@ class ModulesBase:
         self._lib = _lib.lib()
         fam = cfgmod.FAMILIES[self.family]
         if not torch.cuda.is_available():
-            raise _lib.N2NMNError('n2nmn_b200 needs a CUDA (sm_100a) device; there is no CPU path')
+            raise _lib.N2NMNError('n2nmn_b200 needs a CUDA (sm_90a) device; there is no CPU path')
         if device is None:
             device = image_feat_grid.device if isinstance(image_feat_grid, torch.Tensor) and \
                 image_feat_grid.is_cuda else torch.device('cuda', torch.cuda.current_device())

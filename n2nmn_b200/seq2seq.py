@@ -35,7 +35,7 @@ class AttentionSeq2Seq:
                  use_gt_layout=None, gt_layout_batch=None, scope='encoder_decoder', reuse=None,
                  T_encoder=None, max_batch=None, device=None, weights=None, precision='fp32'):
         if encoder_dropout or decoder_dropout:
-            raise NotImplementedError('dropout is a training-time option; the B200 seq2seq is the '
+            raise NotImplementedError('dropout is a training-time option; the H100 seq2seq is the '
                                       'inference configuration')
         self.decoder_sampling = bool(decoder_sampling)
         self.T_decoder = int(T_decoder)
@@ -53,7 +53,7 @@ class AttentionSeq2Seq:
             raise ValueError('give input_seq_batch or T_encoder and max_batch')
         self.device = torch.device(device if device is not None else 'cuda:0')
         if self.device.type != 'cuda':
-            raise _lib.N2NMNError('n2nmn_b200 runs on a CUDA (sm_100) device only')
+            raise _lib.N2NMNError('n2nmn_b200 runs on a CUDA (sm_90) device only')
         self.T_encoder, self.max_batch = int(T_encoder), int(max_batch)
         self._L = _lib.lib()
         cfg = _lib.Seq2SeqConfig(_lib.ABI_VERSION, self.encoder_num_vocab, self.encoder_embed_dim,

@@ -1,6 +1,6 @@
 """GPU parity: the CUDA path (through the C ABI) vs the goldens made from the reference's module
 code and vs the numpy oracle, for all three families, both executors and both projection
-kernels (tcgen05 TF32 default, fp32 CUDA-core verification path).
+kernels (wgmma TF32 default, fp32 CUDA-core verification path).
 
 Tolerance: 1e-3 absolute on attention maps and answer logits (north_star), tightened to 2e-4
 for the fp32 CUDA-core projection."""

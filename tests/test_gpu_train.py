@@ -122,11 +122,13 @@ def test_train_steps_reduce_the_loss():
     assert abs(tr.baseline - 0.5) > 1e-3 and np.isfinite(out['total_loss'])
 
 
-def test_tcgen05_weight_gradient_equals_mma_sync_path_at_batch_64(monkeypatch):
-    """The tcgen05 MN-major weight-gradient kernel (wgrad_umma.cuh) against the mma.sync kernel
-    (xtb_mma_kernel, N2NMN_WGRAD_MMA_SYNC=1) on the BASELINE train batch (64 questions, T=10:
-    ~160 B maps, several entries and weight-set changes per CTA). Both read TF32 operands (one
-    truncates, one rounds): 2e-3 of the largest gradient entry; biases to fp32 accuracy."""
+
+def test_wgmma_weight_gradient_equals_mma_sync_path_at_batch_64(monkeypatch):
+    """The wgmma weight-gradient kernel (wgrad_wgmma.cuh: operands staged transposed into K-major
+    tiles) against the mma.sync kernel (xtb_mma_kernel, N2NMN_WGRAD_MMA_SYNC=1) on the BASELINE
+    train batch (64 questions, T=10: ~160 B maps, several entries and weight-set changes per CTA).
+    Both read TF32 operands (one truncates, one rounds): 2e-3 of the largest gradient entry;
+    biases to fp32 accuracy."""
     N, H, Wd, D, T, Cc = 64, 10, 15, 512, 10, 28
     feat, word_vecs, W, asm, ex, tr = make('clevr', N, H, Wd, D, T, Cc, seed=11)
     tokens = synth.expert_mix_tokens(asm, N, T)

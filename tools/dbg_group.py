@@ -1,5 +1,6 @@
-import numpy as np, torch, sys
-sys.path.insert(0,'/root/repo')
+import os, sys
+import numpy as np, torch
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from n2nmn_b200 import synth, weights as wts, _lib
 from n2nmn_b200.assembler import Assembler
 from n2nmn_b200.executor import LayoutExecutor

@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """Per-launch CUDA-event timing of the three forward kernels when ONE set of launches covers G
-batches (n2nmn_forward_group), G = 1, 2, 4, 8; also the command captured under ncu
-(GB_ONLY=8 GB_ITERS=6 tools/group_bench.py). Env: GB_BATCH, GB_LAYOUT (expert|find), GB_ONLY, GB_ITERS,
+batches (n2nmn_forward_group), G = 1, 2, 4, 8 (GB_ONLY=8: one G only). Env: GB_BATCH, GB_LAYOUT (expert|find), GB_ONLY, GB_ITERS,
 GB_CLUSTER (tree CTAs per question, default 1), GB_TEXT (text CTAs per node group, default 1)."""
 import os, sys
 import numpy as np
@@ -50,7 +49,7 @@ for G in ([int(only)] if only else [1, 2, 4, 8, 16]):
     ex.set_profiling(False)
     med = {k: float(np.median(v)) for k, v in acc.items()}
     fl, by = info['kernel_flops'][1], info['kernel_bytes'][1]
-    pu = med.get('proj_umma_kernel', float('nan'))
+    pu = med.get('proj_wgmma_kernel', float('nan'))
     print('G=%d B=%d %s | us per launch (median): %s | per batch: %s | proj: %.1f TF/s = %.3f of TF32 '
           'peak, %.0f GB/s = %.3f of HBM peak, items %d' % (
               G, B, layout, {k: round(v, 1) for k, v in med.items()},

@@ -25,7 +25,7 @@ __global__ void k(float* out, long long* cyc, int iters) {
 }
 template <int MODE> void run(const char* name, int threads) {
   float* out; long long* cyc;
-  cudaMalloc(&out, 4 * 1024 * 148); cudaMalloc(&cyc, 8 * 148);
+  cudaMalloc(&out, 4 * 1024 * 132); cudaMalloc(&cyc, 8 * 132);
   const int iters = 1000;
   k<MODE><<<1, threads>>>(out, cyc, iters);
   k<MODE><<<1, threads>>>(out, cyc, iters);

@@ -23,7 +23,7 @@ __global__ void k(float* out, long long* cyc, int iters) {
 }
 int main() {
   float* out; long long* cyc;
-  cudaMalloc(&out, 4 * 1024 * 148); cudaMalloc(&cyc, 8 * 148);
+  cudaMalloc(&out, 4 * 1024 * 132); cudaMalloc(&cyc, 8 * 132);
   const int iters = 1000;
   for (int t : {32, 128, 256, 512}) {
     k<<<1, t>>>(out, cyc, iters); k<<<1, t>>>(out, cyc, iters);

@@ -303,6 +303,25 @@ int n2nmn_train_backward(n2nmn_ctx* ctx, const float* feat_dev, const float* wor
                          int num_vocab, const int32_t* labels_host, float invalid_expr_loss,
                          float* scores_dev, float* gflat_dev, float* dword_dev, float* loss_dev,
                          uint8_t* validity_out, void* stream);
+/* n2nmn_train_backward with the answer prior of the VQA training scripts
+ * (exp_vqa/train_vqa_rl_gt_layout.py:101-142: scores = scores_nmn + scores_qpn).
+ *   score_prior_dev (optional) [N,C]: logits added to the module scores before the loss, e.g. the
+ *     output of the caller's question-prior net; scores_dev then holds the sum.
+ *   dscores_dev (optional) [N,C]: d(mean loss)/d(scores), the gradient to backpropagate into that
+ *     net. Scaled by n2nmn_set_grad_scale like dword_dev, because it is not all-reduced.
+ * Loss rule by family: CLEVR / SHAPES charge `invalid_expr_loss` to an invalid layout (its
+ * dscores row is zero); VQA takes the softmax cross-entropy on EVERY row, an invalid layout's
+ * module scores being zeros (its row is CE(prior, label)), and `invalid_expr_loss` is not used.
+ * The VQA family trains at any map_dim; CLEVR / SHAPES (conv Transform) need map_dim <= 512.
+ * Batches whose nodes, B maps (feature-side layer uses) or stored maps exceed what the context
+ * was created for fail with N2NMN_ERR_CAPACITY. n2nmn_train_backward(...) is
+ * n2nmn_train_backward_ex(..., NULL, NULL, stream). */
+int n2nmn_train_backward_ex(n2nmn_ctx* ctx, const float* feat_dev, const float* word_vecs_dev,
+                            const int32_t* tokens_host, int T, int N, const int32_t* vocab_ops,
+                            int num_vocab, const int32_t* labels_host, float invalid_expr_loss,
+                            float* scores_dev, float* gflat_dev, float* dword_dev, float* loss_dev,
+                            uint8_t* validity_out, const float* score_prior_dev, float* dscores_dev,
+                            void* stream);
 /* g += weight_decay * w on the ".../weights" variables (l2_reg, nmn3_model.py:163-166), per-tensor
  * tf.clip_by_norm(g, max_norm) (:137-138), Adam step `step` (1-based, :132), then the updated
  * weights are re-packed into the context. In data-parallel training the caller all-reduces

@@ -102,6 +102,8 @@ SIGNATURES = {
     'n2nmn_load_flat_weights': (C.c_int, [_P, _P, _P]),
     'n2nmn_train_backward': (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int, _P,
                                        C.c_float, _P, _P, _P, _P, _P, _P]),
+    'n2nmn_train_backward_ex': (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int, _P,
+                                          C.c_float, _P, _P, _P, _P, _P, _P, _P, _P]),
     'n2nmn_adam_step': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_float,
                                   C.c_float, C.c_float, C.c_float, _P]),
     'n2nmn_train_finish': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_float,

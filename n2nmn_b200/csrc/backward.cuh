@@ -4,7 +4,11 @@
 // input_0; reduce_min/max split ties equally; l2_normalize takes the constant branch below eps).
 //
 // Structure (DESIGN.md §4b has the measured history):
-//   loss_kernel      : softmax cross-entropy, validity select, d(loss)/d(scores)
+//   loss_kernel      : softmax cross-entropy (+ optional question-prior logits), validity select
+//                      (VQA: cross-entropy on every row), d(loss)/d(scores)
+//   tail_prep_kernel + head_tail_wgmma_kernel + xtb_mma_kernel<TailGradSrc> : answer heads with
+//                      many classes, batched over all roots before the walk: dê = dS·W_outᵀ,
+//                      d(W_out) = Êᵀ·dS, d(b_out)
 //   tree_bwd_kernel  : reverse walk, ONE CTA PER NODE and one launch per depth level from the
 //                      roots down; gradient maps travel through a global [nodes][HW] buffer (a map
 //                      has one consumer, so one writer); recomputes each module's forward
@@ -51,24 +55,37 @@ struct BwdCtx {
   float* dstencil;        // [nodes][HW][Mp] scratch: d(conv_maps output) of a Transform node
   float* gmap;            // [nodes][HWp] d loss / d(attention map of the node), zero-initialised
   const float* phi;       // [score rows][2][Mp] attended features of the Describe-type roots (forward)
+  // many-class heads (C > 32): d loss / d ê of the Describe-type roots, [score rows][Mp], computed
+  // for all roots at once before the walk (tail_prep_kernel + head_tail_wgmma_kernel), with the
+  // fc_eltwise weight gradient (xtb_mma_kernel<TailGradSrc>); nullptr: the walk does both per root
+  const float* dehat;
   GradOffsets go;
 };
 
 // ---- loss ------------------------------------------------------------------------------------
 // One warp per question. loss_acc[0] += per-sample loss, dscores = (softmax - onehot) / NQ for
 // valid questions, 0 otherwise (invalid rows cost the constant invalid_expr_loss).
-__global__ void loss_kernel(const float* __restrict__ scores, const int32_t* __restrict__ labels,
-                            const int32_t* __restrict__ q_ptr, int NQ, int C, float invalid_loss,
-                            float* __restrict__ dscores, float* __restrict__ per_sample,
+// prior (optional, [NQ][C]): logits added to the module scores before the loss and written back
+// into `scores` (the VQA question-prior net, exp_vqa/train_vqa_gt_layout.py:101-121).
+// ce_all: softmax cross-entropy on every row, invalid layouts included (VQA: an invalid layout
+// scores zeros, so its row is CE(prior, label)). dscores_out (optional): out_scale * dscores.
+__global__ void loss_kernel(float* __restrict__ scores, const float* __restrict__ prior,
+                            const int32_t* __restrict__ labels, const int32_t* __restrict__ q_ptr,
+                            int NQ, int C, float invalid_loss, int ce_all,
+                            float* __restrict__ dscores, float* __restrict__ dscores_out,
+                            float out_scale, float* __restrict__ per_sample,
                             float* __restrict__ loss_acc) {
   const int q = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (q >= NQ) return;
   const bool valid = q_ptr[q + 1] > q_ptr[q];
-  const float* s = scores + (size_t)q * C;
+  float* s = scores + (size_t)q * C;
   float* d = dscores + (size_t)q * C;
-  if (!valid) {
-    for (int c = lane; c < C; c += 32) d[c] = 0.f;
+  float* dout = dscores_out ? dscores_out + (size_t)q * C : nullptr;
+  if (prior != nullptr)   // each lane adds and later reads only its own columns
+    for (int c = lane; c < C; c += 32) s[c] += prior[(size_t)q * C + c];
+  if (!valid && !ce_all) {
+    for (int c = lane; c < C; c += 32) { d[c] = 0.f; if (dout) dout[c] = 0.f; }
     if (lane == 0) { per_sample[q] = invalid_loss; atomicAdd(loss_acc, invalid_loss); }
     return;
   }
@@ -83,11 +100,70 @@ __global__ void loss_kernel(const float* __restrict__ scores, const int32_t* __r
   for (int c = lane; c < C; c += 32) {
     const float p = expf(s[c] - mx) * inv;
     d[c] = (p - (c == y ? 1.f : 0.f)) * invn;
+    if (dout) dout[c] = d[c] * out_scale;
   }
   if (lane == 0) {
     const float l = logf(sum) + mx - s[y];
     per_sample[q] = l;
     atomicAdd(loss_acc, l);
+  }
+}
+
+// ---- many-class answer heads: operands of the batched tail backward ----------------------------
+// dÊ = dS·W_outᵀ runs on head_tail_wgmma_kernel (3xTF32, the forward's fp32-parity scheme: dÊ
+// feeds the l2norm backward, whose projection term cancels), d(W_out) = Êᵀ·dS on xtb_mma_kernel.
+// One CTA per question q: root_set[q] = the fc_eltwise set of its Describe-type root (-1: other
+// root or invalid layout); ê[q] = l2norm(τ∘φ0 (∘φ1)) from the forward's φ, zero for the others;
+// dS[q] as hi / lo planes (value, value - trunc_tf32(value)) with row pitch Cp, zero padded;
+// dst[set][q] = the dê row of q for the set of its root, nullptr otherwise.
+__global__ void __launch_bounds__(256)
+tail_prep_kernel(const BwdCtx c, const NodeRec* __restrict__ nodes, const int32_t* __restrict__ q_ptr,
+                 int Cp, int nb, int32_t* __restrict__ root_set, float* __restrict__ ehat,
+                 float* __restrict__ ds_hi, float* __restrict__ ds_lo, float* __restrict__ dehat,
+                 float** __restrict__ dst) {
+  __shared__ float red[32];
+  const int q = blockIdx.x, Mp = c.md.Mp, M = c.md.M, C = c.md.C;
+  int os = -1, text = 0;
+  if (q_ptr[q + 1] > q_ptr[q]) {
+    const NodeRec nd = nodes[q_ptr[q + 1] - 1];
+    os = nd.op == OP_DESCRIBE ? OS_DESCRIBE : nd.op == OP_SAME_PROPERTY ? OS_SAMEPROP : -1;
+    text = nd.text;
+  }
+  if (threadIdx.x == 0) {
+    root_set[q] = os;
+    for (int s = 0; s < NUM_OUT_SETS; ++s) dst[s * nb + q] = (s == os) ? dehat + (size_t)q * Mp : nullptr;
+  }
+  for (int cc = threadIdx.x; cc < Cp; cc += blockDim.x) {
+    const float v = cc < C ? c.dscores[(size_t)q * C + cc] : 0.f;
+    ds_hi[(size_t)q * Cp + cc] = v;
+    ds_lo[(size_t)q * Cp + cc] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
+  }
+  float* eh = ehat + (size_t)q * Mp;
+  if (os < 0) {
+    for (int ch = threadIdx.x; ch < Mp; ch += blockDim.x) eh[ch] = 0.f;
+    return;
+  }
+  const float* ph = c.phi + (size_t)q * 2 * Mp;
+  const float* tau = c.tb.tau + (size_t)text * Mp;
+  float ss = 0.f;
+  for (int ch = threadIdx.x; ch < M; ch += blockDim.x) {
+    const float e = os == OS_SAMEPROP ? ph[ch] * tau[ch] * ph[Mp + ch] : tau[ch] * ph[ch];
+    ss = fmaf(e, e, ss);
+  }
+  ss = block_reduce<0>(ss, red);
+  const float inv = rsqrtf(fmaxf(ss, kEps));
+  for (int ch = threadIdx.x; ch < Mp; ch += blockDim.x) {
+    float e = 0.f;
+    if (ch < M) e = (os == OS_SAMEPROP ? ph[ch] * tau[ch] * ph[Mp + ch] : tau[ch] * ph[ch]) * inv;
+    eh[ch] = e;
+  }
+}
+
+// lo[i] = w[i] - trunc_tf32(w[i]): the remainder plane of a matrix for the 3xTF32 products.
+__global__ void tf32_lo_kernel(const float* __restrict__ w, float* __restrict__ lo, size_t n) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = w[i];
+    lo[i] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
   }
 }
 
@@ -153,7 +229,9 @@ constexpr int kBwdSlicesMax = 8;   // CTAs per splittable node (>= 19 of the 150
 // Two instantiations: kTransform = true handles every op (the stencil backward of Transform keeps
 // ~170 registers busy: one CTA per SM) and runs the levels that contain Transform nodes; false
 // leaves the Transform body out (128 registers, two CTAs per SM) and runs the other levels.
-template <int KS, bool kTransform>
+// kWide: Mp > 512 (the VQA family, KS = 1, no conv Transform): the Find-type case takes two passes
+// over the channels.
+template <int KS, bool kTransform, bool kWide = false>
 __global__ void __launch_bounds__(kNodeThreads, kTransform ? 1 : 2)
 tree_bwd_kernel(const BwdCtx c, const NodeRec* __restrict__ nodes,
                 const int32_t* __restrict__ bwd_nodes, int first,
@@ -261,7 +339,8 @@ tree_bwd_kernel(const BwdCtx c, const NodeRec* __restrict__ nodes,
         const int os = two ? OS_SAMEPROP : OS_DESCRIBE;
         float* phi0 = v; float* phi1 = v + Mp; float* e = v + 2 * Mp; float* de = v + 3 * Mp;
         float* dphi0 = v + 4 * Mp; float* dphi1 = v + 5 * Mp;
-        for (int cc = threadIdx.x; cc < C; cc += blockDim.x) gsc[cc] = c.dscores[(size_t)nd.out * C + cc];
+        if (c.dehat == nullptr)
+          for (int cc = threadIdx.x; cc < C; cc += blockDim.x) gsc[cc] = c.dscores[(size_t)nd.out * C + cc];
         for (int p = threadIdx.x; p < HW; p += blockDim.x) { a0[p] = fin0[p]; if (two) a1[p] = fin1[p]; }
         __syncthreads();
         softmax_inplace(a0, HW, red);
@@ -282,18 +361,27 @@ tree_bwd_kernel(const BwdCtx c, const NodeRec* __restrict__ nodes,
         const float inv = rsqrtf(fmaxf(ss, kEps));
         // dê = Wout·g ; head weight grads with ê (slice 0)
         float dot = 0.f;
-        for (int ch = threadIdx.x; ch < M; ch += blockDim.x) {
-          const float eh = e[ch] * inv;
-          float acc = 0.f;
-          for (int cc = 0; cc < C; ++cc) {
-            acc = fmaf(md.out_w[os][(size_t)ch * C + cc], gsc[cc], acc);
-            if (slice == 0) atomicAdd(c.gflat + c.go.out_w[os] + (size_t)ch * C + cc, eh * gsc[cc]);
+        if (c.dehat != nullptr) {   // dê and the head weight grads were computed before the walk
+          const float* dr = c.dehat + (size_t)nd.out * Mp;
+          for (int ch = threadIdx.x; ch < M; ch += blockDim.x) {
+            const float acc = dr[ch];
+            de[ch] = acc;
+            dot = fmaf(e[ch] * inv, acc, dot);
           }
-          de[ch] = acc;            // holds dê for now
-          dot = fmaf(eh, acc, dot);
+        } else {
+          for (int ch = threadIdx.x; ch < M; ch += blockDim.x) {
+            const float eh = e[ch] * inv;
+            float acc = 0.f;
+            for (int cc = 0; cc < C; ++cc) {
+              acc = fmaf(md.out_w[os][(size_t)ch * C + cc], gsc[cc], acc);
+              if (slice == 0) atomicAdd(c.gflat + c.go.out_w[os] + (size_t)ch * C + cc, eh * gsc[cc]);
+            }
+            de[ch] = acc;            // holds dê for now
+            dot = fmaf(eh, acc, dot);
+          }
+          if (slice == 0)
+            for (int cc = threadIdx.x; cc < C; cc += blockDim.x) atomicAdd(c.gflat + c.go.out_b[os] + cc, gsc[cc]);
         }
-        if (slice == 0)
-          for (int cc = threadIdx.x; cc < C; cc += blockDim.x) atomicAdd(c.gflat + c.go.out_b[os] + cc, gsc[cc]);
         dot = block_reduce<0>(dot, red);
         if (!(ss > kEps)) dot = 0.f;
         float* dtau = c.dtau + (size_t)nd.text * Mp;
@@ -384,8 +472,73 @@ tree_bwd_kernel(const BwdCtx c, const NodeRec* __restrict__ nodes,
         // lane owns channels lane + 32k: the map row is read once into registers, and the
         // per-channel sums over this warp's pixels stay in registers until the end (they used to
         // be one shared-memory atomic per (pixel, channel) with all 8 warps on the same addresses)
-        constexpr int kCh = 16;                 // Mp <= 512 on the training path
+        constexpr int kCh = 16;                 // registers per lane: Mp <= 512 in one pass
         const int nk = Mp >> 5;
+        if constexpr (kWide) {
+          // Mp > 512 (VQA: 1024): a lane's channels do not fit in registers at once. Pass 1 keeps
+          // each pixel's l2norm statistics (1/|e|, ê·w2) in shared memory (da, db_); pass 2 walks
+          // the channels 16 per lane at a time and re-reads the map rows for every group.
+          for (int p = p_lo + warp; p < p_hi; p += nwarps) {
+            const float* mrow = mimg + (size_t)p * Mp;
+            float ss = 0.f, num = 0.f;
+            for (int k0 = 0; k0 < nk; k0 += kCh) {
+              float mv[kCh];
+#pragma unroll
+              for (int k = 0; k < kCh; ++k) mv[k] = (k0 + k < nk) ? __ldg(mrow + (k0 + k) * 32 + lane) : 0.f;
+#pragma unroll
+              for (int k = 0; k < kCh; ++k) {
+                if (k0 + k < nk) {
+                  const int ch = (k0 + k) * 32 + lane;
+                  const float ev = mv[k] * coef[ch];
+                  ss = fmaf(ev, ev, ss);
+                  num = fmaf(ev, w2s[ch], num);
+                }
+              }
+            }
+            ss = warp_sum(ss); num = warp_sum(num);
+            if (lane == 0) {
+              const float inv = rsqrtf(fmaxf(ss, kEps));
+              da[p] = inv;
+              db_[p] = (ss > kEps) ? num * inv : 0.f;
+              db2 += gm[p];
+            }
+          }
+          __syncwarp();   // pass 2 visits the same pixels with the same warp
+          for (int k0 = 0; k0 < nk; k0 += kCh) {
+            float dcoef_r[kCh], dw2_r[kCh];
+#pragma unroll
+            for (int k = 0; k < kCh; ++k) { dcoef_r[k] = 0.f; dw2_r[k] = 0.f; }
+            for (int p = p_lo + warp; p < p_hi; p += nwarps) {
+              const float gp = gm[p], inv = da[p], proj = db_[p];
+              const float* mrow = mimg + (size_t)p * Mp;
+              float mv[kCh];
+#pragma unroll
+              for (int k = 0; k < kCh; ++k) mv[k] = (k0 + k < nk) ? __ldg(mrow + (k0 + k) * 32 + lane) : 0.f;
+#pragma unroll
+              for (int k = 0; k < kCh; ++k) {
+                if (k0 + k < nk) {
+                  const int ch = (k0 + k) * 32 + lane;
+                  float dm = 0.f;
+                  if (ch < M) {
+                    const float eh = mv[k] * coef[ch] * inv;
+                    const float dev = gp * (w2s[ch] - eh * proj) * inv;
+                    dm = dev * coef[ch];
+                    dcoef_r[k] = fmaf(dev, mv[k], dcoef_r[k]);
+                    dw2_r[k] = fmaf(gp, eh, dw2_r[k]);
+                  }
+                  B[(size_t)p * Mp + ch] = dm;
+                }
+              }
+            }
+#pragma unroll
+            for (int k = 0; k < kCh; ++k) {
+              if (k0 + k < nk) {
+                atomicAdd(&dcoef[(k0 + k) * 32 + lane], dcoef_r[k]);
+                atomicAdd(&dw2[(k0 + k) * 32 + lane], dw2_r[k]);
+              }
+            }
+          }
+        } else {   // Mp <= 512: one pass, the lane's channels stay in registers
         float dcoef_r[kCh], dw2_r[kCh];
 #pragma unroll
         for (int k = 0; k < kCh; ++k) { dcoef_r[k] = 0.f; dw2_r[k] = 0.f; }
@@ -434,6 +587,7 @@ tree_bwd_kernel(const BwdCtx c, const NodeRec* __restrict__ nodes,
             atomicAdd(&dw2[k * 32 + lane], dw2_r[k]);
           }
         }
+        }   // kWide
         if (lane == 0) atomicAdd(c.gflat + c.go.elt_b[es], db2);
         __syncthreads();
         float* dtau = c.dtau + (size_t)nd.text * Mp;
@@ -787,6 +941,8 @@ struct FeatGradSrc {   // segment = one B map (entry)
   }
   __device__ const float* b_row(int sg, int p) const { return dmap + ((size_t)sg * md.HW + p) * md.Mp; }
   __device__ int kdim() const { return md.Dk; }
+  __device__ int ncols() const { return md.M; }
+  __device__ int ncols_pad() const { return md.Mp; }
   __device__ float* w_out(int st) const { return gflat + go.proj_w[st]; }
   __device__ float* b_out(int st) const { return gflat + go.proj_b[st]; }
 };
@@ -802,8 +958,29 @@ struct TextGradSrc {   // segment = one text weight set
   }
   __device__ const float* b_row(int sg, int p) const { return dtau + (size_t)(set_start[sg] + p) * md.Mp; }
   __device__ int kdim() const { return md.Dt; }
+  __device__ int ncols() const { return md.M; }
+  __device__ int ncols_pad() const { return md.Mp; }
   __device__ float* w_out(int st) const { return gflat + go.txt_w[st]; }
   __device__ float* b_out(int st) const { return gflat + go.txt_b[st]; }
+};
+// segment = one answer-head weight set (fc_eltwise of Describe / SameProperty, many classes):
+// d(W_out)[m, c] = Σ_q ê[q, m]·dS[q, c] over the questions whose root uses that set; the rows of
+// the other questions read a zero row.
+struct TailGradSrc {
+  DevModel md; const float* ehat; const float* ds; const int32_t* root_set; const float* zero_row;
+  int nq, Cp; float* gflat; GradOffsets go; int has_set[NUM_OUT_SETS];
+  __device__ int num_segs() const { return NUM_OUT_SETS; }
+  __device__ int rows(int sg) const { return has_set[sg] ? nq : 0; }
+  __device__ int set(int sg) const { return sg; }
+  __device__ const float* x_row(int, int p) const { return ehat + (size_t)p * md.Mp; }
+  __device__ const float* b_row(int sg, int p) const {
+    return root_set[p] == sg ? ds + (size_t)p * Cp : zero_row;
+  }
+  __device__ int kdim() const { return md.M; }
+  __device__ int ncols() const { return md.C; }
+  __device__ int ncols_pad() const { return Cp; }
+  __device__ float* w_out(int st) const { return gflat + go.out_w[st]; }
+  __device__ float* b_out(int st) const { return gflat + go.out_b[st]; }
 };
 
 template <class Src>
@@ -813,7 +990,7 @@ __global__ void __launch_bounds__(kXtbThreads) xtb_mma_kernel(const Src src, int
   const int s0 = blockIdx.z * segs_per_cta, s1 = min(src.num_segs(), s0 + segs_per_cta);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3, wm = warp & 3, wn = warp >> 2;
-  const int Kd = src.kdim(), M = src.md.M, Mp = src.md.Mp;
+  const int Kd = src.kdim(), M = src.ncols(), Mp = src.ncols_pad();
   const bool bias_cta = blockIdx.x == 0;
   struct It { int seg, p0; };
   auto settle = [&](It& it) { while (it.seg < s1 && it.p0 >= src.rows(it.seg)) { ++it.seg; it.p0 = 0; } };

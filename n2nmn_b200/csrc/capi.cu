@@ -146,7 +146,16 @@ struct n2nmn_ctx {
   float* dstencil = nullptr;
   float* gmap = nullptr;
   float* phi_buf = nullptr;
-  bool wg_ok = false;   // shapes fit wgrad_wgmma_kernel (Mp == 256, Dk % 128 == 0, no re-pitch)
+  bool wg_ok = false;   // shapes fit wgrad_wgmma_kernel (Mp % 256 == 0, Dk >= 128)
+  // batched answer-tail backward of the many-class heads (C > 32, backward.cuh tail_prep_kernel)
+  float* dehat = nullptr;        // [NB][Mp] d loss / d ê
+  float* ds_hi = nullptr;        // [NB][Cp] d loss / d scores, and its TF32 remainder
+  float* ds_lo = nullptr;
+  float* tail_zero = nullptr;    // max(Cp, Mp) zeros
+  int32_t* root_set = nullptr;   // [NB]
+  float** tail_dst = nullptr;    // [NUM_OUT_SETS][NB] dê row addresses
+  float* out_wp_lo[NUM_OUT_SETS] = {};   // remainder planes of out_wp
+  HeadTailMaps tail_maps[NUM_OUT_SETS];
   // many-class answer heads (C > 32): ê rows + score-row addresses of the roots of a launch, and
   // the fc_eltwise matrices with rows pitched to a multiple of 4 floats (cp.async alignment)
   float* ehat = nullptr;
@@ -883,8 +892,11 @@ int n2nmn_destroy(n2nmn_ctx* c) {
   cudaFree(c->pooled); cudaFree(c->pool_att); cudaFree(c->conv_quad); cudaFree(c->tb.tq);
   cudaFree(c->dscores); cudaFree(c->per_sample); cudaFree(c->dtau); cudaFree(c->dmap); cudaFree(c->dstencil); cudaFree(c->gmap); cudaFree(c->phi_buf);
   cudaFree(c->ehat); cudaFree(c->ehat_dst); cudaFree(c->ehat_lo);
+  cudaFree(c->dehat); cudaFree(c->ds_hi); cudaFree(c->ds_lo); cudaFree(c->tail_zero);
+  cudaFree(c->root_set); cudaFree(c->tail_dst);
   for (int os = 0; os < NUM_OUT_SETS; ++os) {
     cudaFree(c->out_wp[os]); cudaFree(c->out_wt_hi[os]); cudaFree(c->out_wt_lo[os]);
+    cudaFree(c->out_wp_lo[os]);
   }
   cudaFree(c->d_segs); cudaFree(c->d_sumsq);
   cudaFree(c->scores_tmp); cudaFree(c->e2e_feat); cudaFree(c->e2e_wv); cudaFree(c->e2e_scores);
@@ -1481,43 +1493,88 @@ int n2nmn_train_backward(n2nmn_ctx* c, const float* feat_dev, const float* wv_de
                          int num_vocab, const int32_t* labels_host, float invalid_expr_loss,
                          float* scores_dev, float* gflat_dev, float* dword_dev, float* loss_dev,
                          uint8_t* validity_out, void* stream) {
+  return n2nmn_train_backward_ex(c, feat_dev, wv_dev, tokens, T, N, vocab_ops, num_vocab,
+                                 labels_host, invalid_expr_loss, scores_dev, gflat_dev, dword_dev,
+                                 loss_dev, validity_out, nullptr, nullptr, stream);
+}
+
+int n2nmn_train_backward_ex(n2nmn_ctx* c, const float* feat_dev, const float* wv_dev,
+                            const int32_t* tokens, int T, int N, const int32_t* vocab_ops,
+                            int num_vocab, const int32_t* labels_host, float invalid_expr_loss,
+                            float* scores_dev, float* gflat_dev, float* dword_dev, float* loss_dev,
+                            uint8_t* validity_out, const float* score_prior_dev, float* dscores_dev,
+                            void* stream) {
   if (!c || !tokens || !vocab_ops || !labels_host || !scores_dev || !gflat_dev || !loss_dev)
     return fail(N2NMN_ERR_ARG, "null argument");
   if (c->cfg.flags & N2NMN_FLAG_WAVE_EXECUTOR)
     return fail(N2NMN_ERR_ARG, "training uses the tree executor");
-  // The backward walk is instantiated for the 3x3 / 5x5 Transform families and sizes its channel
-  // loops for Mp <= 512 (backward.cuh); the VQA family (no conv Transform, Mp = 1024) has no
-  // backward path yet.
-  if (c->cfg.family == N2NMN_VQA || c->Mp > 512)
-    return fail(N2NMN_ERR_ARG, "n2nmn_train_backward: the VQA family / map_dim > 512 is not supported");
+  // The conv-Transform backward (3x3 / 5x5 filter bank, channels in registers) covers Mp <= 512;
+  // the VQA family has no conv Transform and runs the wide Find-type walk at any map_dim.
+  const bool vqa = c->cfg.family == N2NMN_VQA;
+  if (!vqa && c->Mp > 512)
+    return fail(N2NMN_ERR_ARG,
+                "n2nmn_train_backward: map_dim > 512 is not supported for the conv-Transform families");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = n2nmn_bind_inputs(c, feat_dev, wv_dev, N, T, stream)) return rc;
   if (int rc = check_ready(c)) return rc;
   const int NB = c->cfg.max_batch, TT = c->cfg.max_T, C = c->cfg.num_choices;
+  const int KSb = vqa ? 1 : c->cfg.kernel_size;
+  const bool wide = c->Mp > 512;
   if (!c->dscores) {
     CUDA_TRY(cudaMalloc(&c->dscores, (size_t)NB * C * sizeof(float)));
     CUDA_TRY(cudaMalloc(&c->per_sample, (size_t)NB * sizeof(float)));
     CUDA_TRY(cudaMalloc(&c->dtau, (size_t)c->text_rows_cap * c->Mp * sizeof(float)));
     c->dmap_entries = NB * TT;
     CUDA_TRY(cudaMalloc(&c->dmap, (size_t)c->dmap_entries * c->HW * c->Mp * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->dstencil, (size_t)c->dmap_entries * c->HW * c->Mp * sizeof(float)));
+    if (!vqa)   // d(conv output) scratch of the conv Transform
+      CUDA_TRY(cudaMalloc(&c->dstencil, (size_t)c->dmap_entries * c->HW * c->Mp * sizeof(float)));
     CUDA_TRY(cudaMalloc(&c->gmap, (size_t)c->arena_slots * ((c->HW + 3) & ~3) * sizeof(float)));
     CUDA_TRY(cudaMalloc(&c->phi_buf, (size_t)NB * 2 * c->Mp * sizeof(float)));
-    c->wg_ok = c->Mp == kWgN && c->Dk % kWgM == 0 && !c->feat_aug;
+    c->wg_ok = c->Mp % kWgN == 0 && c->Dk >= kWgM;
     if (c->wg_ok)
       CUDA_TRY(cudaFuncSetAttribute(wgrad_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)kWgSmemBytes));
-    const BwdSmem L = bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, c->cfg.kernel_size, C);
+    if (c->ehat) {   // many-class heads: the batched tail backward
+      const int zeros = std::max(c->Cp, c->Mp);
+      CUDA_TRY(cudaMalloc(&c->dehat, (size_t)NB * c->Mp * sizeof(float)));
+      CUDA_TRY(cudaMalloc(&c->ds_hi, (size_t)NB * c->Cp * sizeof(float)));
+      CUDA_TRY(cudaMalloc(&c->ds_lo, (size_t)NB * c->Cp * sizeof(float)));
+      CUDA_TRY(cudaMalloc(&c->tail_zero, (size_t)zeros * sizeof(float)));
+      CUDA_TRY(cudaMemset(c->tail_zero, 0, (size_t)zeros * sizeof(float)));
+      CUDA_TRY(cudaMalloc(&c->root_set, (size_t)NB * sizeof(int32_t)));
+      CUDA_TRY(cudaMalloc(&c->tail_dst, (size_t)NUM_OUT_SETS * NB * sizeof(float*)));
+      for (int os = 0; os < NUM_OUT_SETS; ++os) {
+        if (!c->out_wp[os]) continue;
+        const size_t n = (size_t)c->cfg.map_dim * c->Cp;
+        CUDA_TRY(cudaMalloc(&c->out_wp_lo[os], n * sizeof(float)));
+        HeadTailMaps& tm = c->tail_maps[os];
+        const int M = c->cfg.map_dim;
+        if (int rc = encode_2d(c, &tm.a_hi, c->ds_hi, c->Cp, NB, c->Cp, kHtK, kHtM)) return rc;
+        if (int rc = encode_2d(c, &tm.a_lo, c->ds_lo, c->Cp, NB, c->Cp, kHtK, kHtM)) return rc;
+        if (int rc = encode_2d(c, &tm.b_hi, c->out_wp[os], c->Cp, M, c->Cp, kHtK, kHtN)) return rc;
+        if (int rc = encode_2d(c, &tm.b_lo, c->out_wp_lo[os], c->Cp, M, c->Cp, kHtK, kHtN)) return rc;
+      }
+    }
+    const BwdSmem L = bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, KSb, C);
     const int bwd_smem = (int)(L.total * sizeof(float));
-    CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-    CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-    CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-    CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-    CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    if (vqa) {
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<1, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<1, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    } else {
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    }
     CUDA_TRY(cudaFuncSetAttribute(xtb_mma_kernel<FeatGradSrc>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kXtbSmemBytes));
     CUDA_TRY(cudaFuncSetAttribute(xtb_mma_kernel<TextGradSrc>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kXtbSmemBytes));
+    CUDA_TRY(cudaFuncSetAttribute(xtb_mma_kernel<TailGradSrc>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kXtbSmemBytes));
     CUDA_TRY(cudaFuncSetAttribute(text_xgrad_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)kXgSmemBytes));
@@ -1567,17 +1624,53 @@ int n2nmn_train_backward(n2nmn_ctx* c, const float* feat_dev, const float* wv_de
   CUDA_TRY(cudaMemsetAsync(loss_dev, 0, sizeof(float), st));
   if (dword_dev)
     CUDA_TRY(cudaMemsetAsync(dword_dev, 0, (size_t)T * N * c->cfg.text_dim * sizeof(float), st));
-  loss_kernel<<<(N + 7) / 8, 256, 0, st>>>(scores_dev, reinterpret_cast<const int32_t*>(d + o.labels),
-                                           d_qptr, N, C, invalid_expr_loss, c->dscores,
-                                           loss_dev + 1, loss_dev);
+  // VQA: cross-entropy on every row (exp_vqa/train_vqa_rl_gt_layout.py:101-116; invalid_expr_loss
+  // only seeds the baseline there)
+  loss_kernel<<<(N + 7) / 8, 256, 0, st>>>(scores_dev, score_prior_dev,
+                                           reinterpret_cast<const int32_t*>(d + o.labels), d_qptr, N,
+                                           C, invalid_expr_loss, vqa ? 1 : 0, c->dscores, dscores_dev,
+                                           c->dword_scale, loss_dev + 1, loss_dev);
   ++c->launches;
   prof_mark(c, "loss_kernel", st);
-  // ---- reverse tree walk
   BwdCtx bc;
   bc.md = c->md; bc.tb = c->tb; bc.arena = c->arena; bc.scores = scores_dev;
   bc.dscores = c->dscores; bc.mbuf = c->mbuf; bc.gflat = gflat_dev; bc.dtau = c->dtau;
   bc.dmap = c->dmap; bc.dstencil = c->dstencil; bc.gmap = c->gmap; bc.phi = c->phi_buf; bc.go = c->go;
-  const BwdSmem L = bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, c->cfg.kernel_size, C);
+  bc.dehat = nullptr;
+  // ---- many-class heads: dê of every Describe-type root and the fc_eltwise gradients, batched
+  // (the exact-fp32 verification path keeps the per-root CUDA-core loop of the walk)
+  if (c->ehat && !(c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT)) {
+    tail_prep_kernel<<<N, 256, 0, st>>>(bc, d_nodes, d_qptr, c->Cp, NB, c->root_set, c->ehat,
+                                        c->ds_hi, c->ds_lo, c->dehat, c->tail_dst);
+    ++c->launches;
+    prof_mark(c, "tail_prep_kernel", st);
+    TailGradSrc ts;
+    ts.md = c->md; ts.ehat = c->ehat; ts.ds = c->ds_hi; ts.root_set = c->root_set;
+    ts.zero_row = c->tail_zero; ts.nq = N; ts.Cp = c->Cp; ts.gflat = gflat_dev; ts.go = c->go;
+    for (int os = 0; os < NUM_OUT_SETS; ++os) {
+      ts.has_set[os] = c->out_wp[os] != nullptr;
+      if (!c->out_wp[os]) continue;
+      const size_t n = (size_t)c->cfg.map_dim * c->Cp;
+      tf32_lo_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, 4 * (size_t)c->num_sms), 256, 0, st>>>(
+          c->out_wp[os], c->out_wp_lo[os], n);
+      // dÊ[q, :] = dS[q, :]·W_outᵀ for the questions whose root uses this set (3xTF32)
+      head_tail_wgmma_kernel<<<dim3((unsigned)((c->cfg.map_dim + kHtN - 1) / kHtN),
+                                    (unsigned)((N + kHtM - 1) / kHtM)),
+                               kHtThreads, kHtSmemBytes, st>>>(
+          c->tail_maps[os], c->tail_zero, c->tail_dst + (size_t)os * NB, 0, N, c->cfg.map_dim, C);
+      c->launches += 2;
+    }
+    prof_mark(c, "tail_dehat_kernel", st);
+    // d(W_out) = Êᵀ·dS and d(b_out) = Σ_q dS, one segment per weight set
+    dim3 gt((c->cfg.map_dim + kXtbM - 1) / kXtbM, (C + kXtbN - 1) / kXtbN, NUM_OUT_SETS);
+    xtb_mma_kernel<TailGradSrc><<<gt, kXtbThreads, kXtbSmemBytes, st>>>(ts, 1);
+    ++c->launches;
+    CUDA_TRY(cudaGetLastError());
+    prof_mark(c, "tail_wgrad_kernel", st);
+    bc.dehat = c->dehat;
+  }
+  // ---- reverse tree walk
+  const BwdSmem L = bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, KSb, C);
   const size_t bsm = L.total * sizeof(float);
   const int32_t* d_entry = reinterpret_cast<const int32_t*>(d + o.node_entry);
   const int32_t* d_bwd = reinterpret_cast<const int32_t*>(d + o.bwd_nodes);
@@ -1606,7 +1699,10 @@ int n2nmn_train_backward(n2nmn_ctx* c, const float* feat_dev, const float* wv_de
     bl.attrs = battr;
     bl.numAttrs = c->use_pdl ? 1 : 0;
     const bool k5 = c->cfg.kernel_size == 5;
-    if (has_tr) {
+    if (vqa) {
+      if (wide) CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<1, false, true>, bc, d_nodes, d_bwd, first, d_entry));
+      else CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<1, false, false>, bc, d_nodes, d_bwd, first, d_entry));
+    } else if (has_tr) {
       if (k5) CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<5, true>, bc, d_nodes, d_bwd, first, d_entry));
       else CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<3, true>, bc, d_nodes, d_bwd, first, d_entry));
     } else {
@@ -1662,15 +1758,22 @@ int n2nmn_train_backward(n2nmn_ctx* c, const float* feat_dev, const float* wv_de
       feat_grad_kernel<<<g2, 256, 0, st>>>(c->md, c->dmap, d_ent, ne, per, gflat_dev, c->go);
     } else if (c->wg_ok && !std::getenv("N2NMN_WGRAD_MMA_SYNC")) {
       // wgmma, both operands staged transposed (K-major) from the feature grid and the B maps
-      const int slabs = c->Dk / kWgM;
-      const int chunks = std::max(1, std::min(ne, c->num_sms / slabs));
+      const int slabs = (c->Dk + kWgM - 1) / kWgM, ntiles = c->Mp / kWgN, tiles = slabs * ntiles;
+      int chunks = std::max(1, std::min(ne, c->num_sms / tiles));
+      if (chunks < 4) {   // few entry chunks per tile: pick the count that wastes the least of the waves
+        double best = 1e30;
+        for (int k = 1; k <= std::min(ne, 8); ++k) {
+          const double cost = (double)((tiles * k + c->num_sms - 1) / c->num_sms) / k;
+          if (cost < best - 1e-9) { best = cost; chunks = k; }
+        }
+      }
       WgradParams wp;
       wp.feat = c->md.feat; wp.dmap = c->dmap; wp.entries = d_ent;
       wp.order = reinterpret_cast<const int32_t*>(d + o.entry_order);
       wp.num_entries = ne; wp.per_cta = (ne + chunks - 1) / chunks;
       wp.HW = c->HW; wp.Dk = c->Dk; wp.M = c->cfg.map_dim; wp.Mp = c->Mp;
       wp.pitch = c->md.feat_pitch; wp.gflat = gflat_dev; wp.go = c->go;
-      dim3 gw(slabs, (ne + wp.per_cta - 1) / wp.per_cta);
+      dim3 gw(slabs, (ne + wp.per_cta - 1) / wp.per_cta, ntiles);
       wgrad_wgmma_kernel<<<gw, kWgThreads, kWgSmemBytes, st>>>(wp);
       prof_mark(c, "feat_grad_kernel", st);
       bmap_colsum_kernel<<<ne, 1024, 0, st>>>(c->dmap, d_ent, c->HW, c->cfg.map_dim, c->Mp, gflat_dev,

@@ -7,10 +7,13 @@
 // channels) with coalesced 16-byte loads and store them as K-major 128B-swizzled tiles
 // Xᵀ [128 rows k][32 p] and Bᵀ [256 rows c][32 p] (the layout TMA's SWIZZLE_128B would write).
 // The global loads of stage s+1 are issued before waiting on the wgmma of stage s.
-//   CTA = one 128-feature slab of k x all 256 channels x a chunk of the entries (sorted by weight
-//   set by the host), 256 threads = 2 warpgroups of 64 features each: wgmma.m64n256k8, 4 per
-//   stage; the accumulator is flushed with float2 reductions when the weight set changes and at
-//   the end. Pixels >= H·W are zero.
+//   CTA = one 128-feature slab of k x one 256-channel tile (blockIdx.z; Mp is a multiple of 256)
+//   x a chunk of the entries (sorted by weight set by the host), 256 threads = 2 warpgroups of 64
+//   features each: wgmma.m64n256k8, 4 per stage; the accumulator is flushed with float2
+//   reductions when the weight set changes and at the end. Pixels >= H·W are zero, and so are the
+//   features k >= Dk of a ragged last slab (VQA: Dk = 2050, the two coordinate channels last);
+//   their gradient rows are not written. The feature rows are read at their pitch (the
+//   coordinate-augmented / re-pitched copy of the forward pass, or the caller's grid).
 // Operands are the fp32 bits read as TF32 (as in the forward contraction); fp32 accumulate.
 #pragma once
 #include "backward.cuh"
@@ -45,7 +48,7 @@ wgrad_wgmma_kernel(const WgradParams p) {
   float* sa = reinterpret_cast<float*>(smem);                 // Xᵀ [128][32]
   float* sb = reinterpret_cast<float*>(smem + kWgABytes);     // Bᵀ [256][32]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, t = tid & 127;
-  const int k0 = blockIdx.x * kWgM;
+  const int k0 = blockIdx.x * kWgM, n0 = blockIdx.z * kWgN;
   const int e0 = blockIdx.y * p.per_cta, e1 = min(p.num_entries, e0 + p.per_cta);
   const int stages_per_entry = (p.HW + kWgP - 1) / kWgP;
   const int n_stages = (e1 > e0 ? e1 - e0 : 0) * stages_per_entry;
@@ -57,12 +60,13 @@ wgrad_wgmma_kernel(const WgradParams p) {
     const int e = p.order[e0 + s / stages_per_entry];
     const int p0 = (s % stages_per_entry) * kWgP;
     const float* X = p.feat + (size_t)p.entries[e].b * p.HW * p.pitch + k0;
-    const float* B = p.dmap + (size_t)e * p.HW * p.Mp;
+    const float* B = p.dmap + (size_t)e * p.HW * p.Mp + n0;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {   // 32 pixels x 32 quads of 128 features
       const int px = p0 + i * 8 + p_lo, q = warp * 4 + q_lo;
-      xa[i] = px < p.HW ? __ldg(reinterpret_cast<const float4*>(X + (size_t)px * p.pitch) + q)
-                        : make_float4(0.f, 0.f, 0.f, 0.f);
+      xa[i] = (px < p.HW && k0 + 4 * q < p.Dk)
+                  ? __ldg(reinterpret_cast<const float4*>(X + (size_t)px * p.pitch) + q)
+                  : make_float4(0.f, 0.f, 0.f, 0.f);
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {   // 32 pixels x 64 quads of 256 channels
@@ -99,7 +103,7 @@ wgrad_wgmma_kernel(const WgradParams p) {
       if (k >= p.Dk) continue;
 #pragma unroll
       for (int j = 0; j < kWgN / 8; ++j) {
-        const int col = 8 * j + 2 * q;
+        const int col = n0 + 8 * j + 2 * q;
         const float a = acc[4 * j + 2 * h], b = acc[4 * j + 2 * h + 1];
         float* dst = W + (size_t)k * p.M + col;
         if (pair_ok && col + 1 < p.M) {

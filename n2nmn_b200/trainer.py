@@ -7,6 +7,13 @@
     total    = pg + avg + 0.005 * entropy_reg + 5e-6 * l2_reg                              (:126-129)
     Adam(1e-4) on per-tensor clip_by_norm(grad, 10)                                        (:132-139)
 
+VQA (exp_vqa/train_vqa{,2}_{gt,rl_gt}_layout.py:101-142) differs in two places: the scores are
+`scores_nmn + scores_qpn`, the logits of a question-prior net the caller owns (`score_prior`;
+`d_scores` comes back for its backward pass), and loss_i is the cross-entropy on EVERY row (an
+invalid layout's module scores are zeros, so its loss is CE(prior, label)): `invalid_expr_loss`
+only seeds the baseline. The VQA scripts use weight_decay 0 and clip at 10 (rl) or not at all (gt):
+set them on the trainer.
+
 The module network receives gradient only through `avg` and the l2 term; `pg` and the entropy term
 reach the seq2seq layout generator, which is off the hot path: this class returns what that
 generator needs (d total/d word_vecs and the per-sample REINFORCE coefficients) instead of
@@ -105,30 +112,47 @@ class ModuleNetTrainer:
 
     # -- one step ---------------------------------------------------------------------------------
     def forward_backward(self, image_feat_grid, word_vecs, layout_tokens, labels,
-                         want_dword=True):
+                         want_dword=True, score_prior=None):
         """Forward + backward of this rank's shard. Fills self.g (gradient of the LOCAL mean loss)
-        and returns (scores, validity, per_sample_loss tensor, d_word_vecs or None)."""
+        and returns (scores, validity, per_sample_loss tensor, d_word_vecs or None).
+        score_prior: optional [N, num_choices] CUDA logits added to the module scores before the
+        loss (VQA's question-prior net); the returned scores are then the sum, and a fifth
+        element d_scores = d(mean loss)/d(scores) [N, num_choices] follows, scaled by 1/world
+        like d_word_vecs."""
         m = self.m
         tok = np.ascontiguousarray(layout_tokens, dtype=np.int32)
         T, N = tok.shape
         lab = np.ascontiguousarray(labels, dtype=np.int32)
         assert lab.shape == (N,)
-        scores = torch.empty((N, self.ex.num_choices), dtype=torch.float32, device=m.device)
+        nc = self.ex.num_choices
+        scores = torch.empty((N, nc), dtype=torch.float32, device=m.device)
         dword = torch.empty((T, N, m.text_dim), dtype=torch.float32, device=m.device) \
             if want_dword else None
+        prior = dscores = None
+        if score_prior is not None:
+            prior = score_prior.to(m.device, torch.float32).contiguous()
+            if tuple(prior.shape) != (N, nc):
+                raise ValueError('score_prior must be [N, num_choices] = [%d, %d], got %r'
+                                 % (N, nc, tuple(prior.shape)))
+            dscores = torch.empty((N, nc), dtype=torch.float32, device=m.device)
         validity = np.empty(N, np.uint8)
         m.image_feat_grid, m.word_vecs, m.N, m.T = image_feat_grid, word_vecs, N, T
-        _lib.check(self._lib.n2nmn_train_backward(
+        _lib.check(self._lib.n2nmn_train_backward_ex(
             m._h, image_feat_grid.data_ptr(), word_vecs.data_ptr(), tok.ctypes.data, T, N,
             self.ex._vocab_ptr, len(self.ex.vocab_ops), lab.ctypes.data,
             C.c_float(self.invalid_expr_loss), scores.data_ptr(), self.g.data_ptr(),
             dword.data_ptr() if dword is not None else None, self._loss.data_ptr(),
-            validity.ctypes.data, torch.cuda.current_stream(m.device).cuda_stream))
+            validity.ctypes.data, prior.data_ptr() if prior is not None else None,
+            dscores.data_ptr() if dscores is not None else None,
+            torch.cuda.current_stream(m.device).cuda_stream))
+        if prior is not None:
+            return scores, validity.view(bool), self._loss[1:1 + N], dword, dscores
         return scores, validity.view(bool), self._loss[1:1 + N], dword
 
     def train_step(self, image_feat_grid, word_vecs, layout_tokens, labels, log_seq_prob=None,
-                   entropy_reg=0.0, sync=True):
-        """One optimiser step. Returns a dict with the reference's logged quantities."""
+                   entropy_reg=0.0, sync=True, score_prior=None):
+        """One optimiser step. Returns a dict with the reference's logged quantities; with a
+        score_prior (see forward_backward) it also carries 'd_scores'."""
         import torch.distributed as dist
         world = 1
         if dist.is_available() and dist.is_initialized() and dist.get_world_size(self.pg) > 1:
@@ -136,8 +160,9 @@ class ModuleNetTrainer:
         if world != self._world_set:       # d_word_vecs is the one gradient no all-reduce averages
             _lib.check(self._lib.n2nmn_set_grad_scale(self.m._h, C.c_float(1.0 / world)))
             self._world_set = world
-        scores, validity, per_sample, dword = self.forward_backward(
-            image_feat_grid, word_vecs, layout_tokens, labels)
+        res = self.forward_backward(image_feat_grid, word_vecs, layout_tokens, labels,
+                                    score_prior=score_prior)
+        scores, validity, per_sample, dword = res[:4]
         N = scores.shape[0]
         if world > 1:
             dist.all_reduce(self.g, op=dist.ReduceOp.SUM, group=self.pg)   # the ONE collective
@@ -159,6 +184,8 @@ class ModuleNetTrainer:
         st = self._state[cur]
         out = {'scores': scores, 'validity': validity, 'd_word_vecs': dword,
                'reinforce_coeff': self._coeff[cur, :N]}
+        if score_prior is not None:
+            out['d_scores'] = res[4]
         if sync:
             base, avg, pg, l2 = st.tolist()                      # the step's only host read
         else:

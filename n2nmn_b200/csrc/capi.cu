@@ -457,7 +457,27 @@ int run_tables(n2nmn_ctx* c, n2nmn_sched* sc, float* const* scores_seg, float* a
     p.mbuf = c->mbuf;
     // persistent grid: CTA i walks the tiles i, i + CTAs, ... (two tiles per work item)
     const int max_ctas = c->proj_max_ctas > 0 ? std::min(c->proj_max_ctas, c->num_sms) : c->num_sms;
+#if defined(N2NMN_EXP_PROJ_PAIRS)
+    // experiment build (proj_wgmma.cuh): an even grid of 2-CTA clusters, at most what fits at once
+    static int max_pairs = 0;
+    if (max_pairs == 0) {
+      cudaLaunchConfig_t oc;
+      std::memset(&oc, 0, sizeof(oc));
+      oc.gridDim = dim3((unsigned)(2 * (c->num_sms / 2)));
+      oc.blockDim = dim3(kProjThreads);
+      oc.dynamicSmemBytes = proj_smem_bytes();
+      cudaLaunchAttribute ca[1];
+      ca[0].id = cudaLaunchAttributeClusterDimension;
+      ca[0].val.clusterDim.x = 2; ca[0].val.clusterDim.y = 1; ca[0].val.clusterDim.z = 1;
+      oc.attrs = ca;
+      oc.numAttrs = 1;
+      CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, proj_wgmma_kernel, &oc));
+      if (max_pairs < 1) return fail(N2NMN_ERR_CUDA, "no 2-CTA cluster of the projection kernel fits");
+    }
+    const int ctas = 2 * std::max(1, std::min({p.num_work, max_ctas / 2, max_pairs}));
+#else
     const int ctas = std::max(1, std::min(2 * p.num_work, max_ctas));
+#endif
     if (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) {
       const size_t smem = (size_t)(kSimtRows * kSimtKChunk + kSimtRows * c->Mp) * sizeof(float);
       proj_simt_kernel<<<2 * p.num_work, 256, smem, st>>>(p);
@@ -469,11 +489,20 @@ int run_tables(n2nmn_ctx* c, n2nmn_sched* sc, float* const* scores_seg, float* a
       lc.blockDim = dim3(kProjThreads);
       lc.dynamicSmemBytes = proj_smem_bytes();
       lc.stream = st;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[0].val.programmaticStreamSerializationAllowed = 1;
+      cudaLaunchAttribute attr[2];
+      int na = 0;
+#if defined(N2NMN_EXP_PROJ_PAIRS)
+      attr[na].id = cudaLaunchAttributeClusterDimension;
+      attr[na].val.clusterDim.x = 2; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
+      ++na;
+#endif
+      if (pdl_ok()) {
+        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[na].val.programmaticStreamSerializationAllowed = 1;
+        ++na;
+      }
       lc.attrs = attr;
-      lc.numAttrs = pdl_ok() ? 1 : 0;
+      lc.numAttrs = na;
       CUDA_TRY(cudaLaunchKernelEx(&lc, proj_wgmma_kernel, c->tmaps, p));
       prof_mark(c, "proj_wgmma_kernel", st);
     }

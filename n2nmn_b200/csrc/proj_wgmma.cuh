@@ -51,6 +51,31 @@ struct ProjTensorMaps {
   CUtensorMap b[NUM_PROJ_SETS];      // W^T [Mp, Kp] fp32 (K-major), box 32 x 128 (half an N-tile)
 };
 
+// Experiment builds (tools/build_variants.py attrib; never the default library) that remove one
+// part of the kernel's work to attribute its time. Their outputs are wrong by design.
+//   N2NMN_EXP_PROJ_NO_EPI  consumers skip the epilogue (bias, stored maps, Find consumers)
+//   N2NMN_EXP_PROJ_NO_STORE  the epilogue writes no stored maps
+//   N2NMN_EXP_PROJ_NO_FIND   the epilogue skips the fused Find consumers
+//   N2NMN_EXP_PROJ_NO_B    the producer streams only the feature box; the MMA reads stale weights
+//   N2NMN_EXP_PROJ_NO_MMA  consumers wait for and release every stage without issuing wgmma
+//   N2NMN_EXP_PROJ_PAIRS   (results stay exact) the grid runs as 2-CTA clusters: CTA r of a
+//                          cluster takes half r of every work item it visits (blockIdx.x =
+//                          2 * cluster + r keeps the tile walk below), fetches weight box r (128
+//                          of the 256 columns) and multicasts it into both CTAs' stage, so each
+//                          CTA pulls 32 KB per stage from L2 instead of 48 KB. A stage is refilled
+//                          once the consumers of both CTAs have released it (16 arrivals), and a
+//                          filler half runs the ring and the MMA for its partner, writing nothing.
+#if defined(N2NMN_EXP_PROJ_PAIRS)
+constexpr bool kPair = true;
+#else
+constexpr bool kPair = false;
+#endif
+#if defined(N2NMN_EXP_PROJ_NO_B)
+constexpr int kStageTxBytes = kABytes;
+#else
+constexpr int kStageTxBytes = kStageBytes;
+#endif
+
 __global__ void __launch_bounds__(kProjThreads, 1)
 proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p) {
   extern __shared__ __align__(1024) uint8_t proj_smem_raw[];
@@ -63,6 +88,7 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;   // 0 = producer, 1..2 = consumers
   const int n_tiles_total = 2 * p.num_work;
+  const uint32_t rank = kPair ? ptx::cluster_ctarank() : 0u;
   pdl_trigger();   // let the node kernel's CTAs start prefetching their parameters
 
   if (threadIdx.x == 0) {
@@ -71,11 +97,12 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
     for (int i = 0; i < NUM_PROJ_SETS; ++i) ptx::prefetch_tensormap(&tm.b[i]);
     for (int s = 0; s < kProjStages; ++s) {
       ptx::mbar_init(&full[s], 1);   // the producer's arrive.expect_tx
-      ptx::mbar_init(&empty[s], 8);  // one arrive per consumer warp
+      ptx::mbar_init(&empty[s], kPair ? 16 : 8);  // one arrive per consumer warp (of both CTAs)
     }
     ptx::fence_barrier_init();
   }
-  __syncthreads();
+  if (kPair) ptx::cluster_sync();   // the partner must see the barriers initialised
+  else __syncthreads();
 
   if (wg == 0) {
     // ===================================================================== TMA producer
@@ -86,22 +113,32 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
       for (int ti = blockIdx.x; ti < n_tiles_total; ti += gridDim.x) {
         const ProjWork* wk = p.work + (ti >> 1);
         const int hf = ti & 1;
-        if (wk->pass[hf] < 0) continue;
+        if (!kPair && wk->pass[hf] < 0) continue;
         const int row0 = wk->row0[hf], seg = wk->seg[hf], set = wk->set;
         for (int nt = 0; nt < p.n_tiles; ++nt) {
           for (int kb = 0; kb < p.k_blocks; ++kb) {
             ptx::mbar_wait(&empty[stage], phase ^ 1);
-            ptx::mbar_arrive_expect_tx(&full[stage], kStageBytes);
+            ptx::mbar_arrive_expect_tx(&full[stage], kStageTxBytes);
             uint8_t* dst = smem + stage * kStageBytes;
             ptx::tma_load_2d(dst, &tm.a[seg], kb * kBK, row0, &full[stage]);
-            ptx::tma_load_2d(dst + kABytes, &tm.b[set], kb * kBK, nt * kBN, &full[stage]);
-            ptx::tma_load_2d(dst + kABytes + kBNHalf * kBK * 4, &tm.b[set], kb * kBK,
-                             nt * kBN + kBNHalf, &full[stage]);
+#if !defined(N2NMN_EXP_PROJ_NO_B)
+            if (kPair) {
+              ptx::tma_load_2d_multicast(dst + kABytes + rank * (kBNHalf * kBK * 4), &tm.b[set],
+                                         kb * kBK, nt * kBN + rank * kBNHalf, &full[stage], 0x3);
+            } else {
+              ptx::tma_load_2d(dst + kABytes, &tm.b[set], kb * kBK, nt * kBN, &full[stage]);
+              ptx::tma_load_2d(dst + kABytes + kBNHalf * kBK * 4, &tm.b[set], kb * kBK,
+                               nt * kBN + kBNHalf, &full[stage]);
+            }
+#endif
             if (++stage == kProjStages) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
+    // no CTA of a pair leaves while its partner may still write into its ring or arrive on its
+    // barriers
+    if (kPair) ptx::cluster_sync();
     return;
   }
 
@@ -113,14 +150,24 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
   // tauw / tau2 come from the text-projection kernel, which may still be running (PDL); the
   // producer never touches its output and starts immediately.
   pdl_wait();
+  auto release = [&](int s) {   // one arrive per consumer warp (and on the partner's barrier)
+    if (lane == 0) {
+      ptx::mbar_arrive(&empty[s]);
+      if (kPair) ptx::mbar_arrive_cluster(&empty[s], rank ^ 1u);
+    }
+  };
   int stage = 0;
   uint32_t phase = 0;
   float acc[kBN / 2];
+#if defined(N2NMN_EXP_PROJ_NO_MMA)
+#pragma unroll
+  for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
+#endif
   for (int ti = blockIdx.x; ti < n_tiles_total; ti += gridDim.x) {
     const ProjWork* wkp = p.work + (ti >> 1);
     const int hf = ti & 1;
     const int pass = wkp->pass[hf];
-    if (pass < 0) continue;
+    if (!kPair && pass < 0) continue;
     const int row0 = wkp->row0[hf], set = wkp->set;
     const int g0 = wkp->seg[hf] * p.seg_images;   // first image of this tile's segment
     // the two rows of this thread and their consumers
@@ -129,7 +176,7 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = row0 + rbase + 8 * h;
-      const bool row_ok = row < p.total_rows;
+      const bool row_ok = pass >= 0 && row < p.total_rows;   // (a filler half has none)
       const int b = row_ok ? row / p.HW : 0;
       pix[h] = row - b * p.HW;
       e_beg[h] = 0;
@@ -151,6 +198,9 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
       // ---- mainloop: 4 wgmma per stage; a stage is released once the next one's are issued
       for (int kb = 0; kb < p.k_blocks; ++kb) {
         ptx::mbar_wait(&full[stage], phase);
+#if defined(N2NMN_EXP_PROJ_NO_MMA)
+        release(stage);
+#else
         const uint32_t sa = ptx::smem_u32(smem + stage * kStageBytes);
         const uint64_t da = ptx::make_smem_desc_sw128(sa + (wg - 1) * 64 * 128);
         const uint64_t db = ptx::make_smem_desc_sw128(sa + kABytes);
@@ -160,14 +210,42 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
         for (int k = 0; k < kBK / kWgmmaK; ++k)   // 32 bytes (2 x 16-byte units) along K
           ptx::wgmma_m64n256k8_tf32(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
         ptx::wgmma_commit();
+#if !defined(N2NMN_EXP_PROJ_NO_EPI) && !defined(N2NMN_EXP_PROJ_NO_FIND)
+        if (kb == 0 && set == PS_FIND) {
+          // While the first slice's MMAs run: pull the text rows the epilogue reads (this N-tile's
+          // columns of tauw / tau2 for every consumer node of the thread's two rows, 8 lines per
+          // row, 2 per thread of the quad) into L1, so that the rolled node loop below finds
+          // them there instead of waiting on L2 for each node in turn.
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (n_nodes[h] > 0) ptx::prefetch_l1(p.node_out + e_beg[h]);
+#pragma unroll
+            for (int jn = 0; jn < kMaxProjNodesPerPass; ++jn) {
+              if (jn < n_nodes[h]) {
+                const size_t off = (size_t)p.node_text[e_beg[h] + jn] * p.Mp + nt * kBN + 32 * q;
+                ptx::prefetch_l1(p.tauw + off);
+                ptx::prefetch_l1(p.tauw + off + 128);
+                ptx::prefetch_l1(p.tau2 + off);
+                ptx::prefetch_l1(p.tau2 + off + 128);
+              }
+            }
+          }
+        }
+#endif
         ptx::wgmma_wait<1>();
         ptx::fence_regs(acc);
-        if (kb > 0 && lane == 0) ptx::mbar_arrive(&empty[stage == 0 ? kProjStages - 1 : stage - 1]);
+        if (kb > 0) release(stage == 0 ? kProjStages - 1 : stage - 1);
+#endif
         if (++stage == kProjStages) { stage = 0; phase ^= 1; }
       }
+#if !defined(N2NMN_EXP_PROJ_NO_MMA)
       ptx::wgmma_wait<0>();
       ptx::fence_regs(acc);
-      if (lane == 0) ptx::mbar_arrive(&empty[stage == 0 ? kProjStages - 1 : stage - 1]);
+      release(stage == 0 ? kProjStages - 1 : stage - 1);
+#endif
+#if defined(N2NMN_EXP_PROJ_NO_EPI)
+      continue;
+#endif
 
       // ---- epilogue on the accumulator: + bias, stored map, fused Find consumers
       const int colq = nt * kBN + 2 * q;   // + 8 j: columns of registers 4j .. 4j+3
@@ -177,6 +255,7 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
         acc[4 * j + 0] += bb.x; acc[4 * j + 1] += bb.y;
         acc[4 * j + 2] += bb.x; acc[4 * j + 3] += bb.y;
       }
+#if !defined(N2NMN_EXP_PROJ_NO_STORE)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (mdst[h] != nullptr) {
@@ -186,6 +265,10 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
                 make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
       }
+#endif
+#if defined(N2NMN_EXP_PROJ_NO_FIND)
+      continue;
+#endif
       if (set != PS_FIND) continue;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -201,13 +284,26 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
             const size_t off = (size_t)p.node_text[e_beg[h] + jn] * p.Mp + colq;
             const float* tw = p.tauw + off;
             const float* t2 = p.tau2 + off;
+            // One text row at a time, all 32 of its loads in flight before the first FMA (the
+            // accumulator leaves room for one row, not two). The squares m² are formed here,
+            // inside the node loop: hoisted out of it they would hold 64 registers and leave
+            // room for only 2-3 loads in flight, i.e. ~25 serial load round-trips per node.
+            float2 w[kBN / 8];
+#pragma unroll
+            for (int j = 0; j < kBN / 8; ++j) w[j] = __ldg(reinterpret_cast<const float2*>(tw + 8 * j));
 #pragma unroll
             for (int j = 0; j < kBN / 8; ++j) {
-              const float2 a = __ldg(reinterpret_cast<const float2*>(tw + 8 * j));
-              const float2 s = __ldg(reinterpret_cast<const float2*>(t2 + 8 * j));
-              const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-              n0 = fmaf(v0, a.x, n0); n1 = fmaf(v1, a.y, n1);
-              d0 = fmaf(v0 * v0, s.x, d0); d1 = fmaf(v1 * v1, s.y, d1);
+              n0 = fmaf(acc[4 * j + 2 * h], w[j].x, n0);
+              n1 = fmaf(acc[4 * j + 2 * h + 1], w[j].y, n1);
+            }
+#pragma unroll
+            for (int j = 0; j < kBN / 8; ++j) w[j] = __ldg(reinterpret_cast<const float2*>(t2 + 8 * j));
+#pragma unroll
+            for (int j = 0; j < kBN / 8; ++j) {
+              float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+              asm volatile("" : "+f"(v0), "+f"(v1));   // keeps v² in the loop
+              d0 = fmaf(v0 * v0, w[j].x, d0);
+              d1 = fmaf(v1 * v1, w[j].y, d1);
             }
           }
           float n = n0 + n1, d = d0 + d1;
@@ -224,6 +320,7 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
       }
     }
     // the N-tiles of a row meet here (the same thread wrote every partial sum it reads)
+#if !defined(N2NMN_EXP_PROJ_NO_EPI) && !defined(N2NMN_EXP_PROJ_NO_FIND)
     if (set == PS_FIND && q == 0) {
       const float b2 = __ldg(p.elt_b);
 #pragma unroll
@@ -235,7 +332,9 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
         }
       }
     }
+#endif
   }
+  if (kPair) ptx::cluster_sync();
 }
 
 }  // namespace n2nmn

@@ -253,10 +253,12 @@ int finalize_schedule(const SchedShape& shp, int images_per_seg, HostSchedule* o
   // Tiles (128 rows of one segment x one layer x one pass of <= 8 Find consumers) in tile-major
   // order: the layers that need the same 128 rows of features are handed out at about the same
   // time, so the A tile is fetched from HBM once and the other layers hit it in L2 (matters once
-  // the batch no longer fits in L2). The kernel runs CTA pairs (cta_group::2): two tiles of the
-  // SAME layer form one work item — they share only the weight matrix, so a tile is paired with the
-  // next tile of its layer wherever that one comes from. A layer with an odd tile count gets a
-  // filler half (pass = -1: the MMA runs on a repeated tile, nothing is written).
+  // the batch no longer fits in L2). Two tiles of the SAME layer form one work item; the default
+  // kernel's persistent CTAs walk single tiles, and the pairing lets a 2-CTA cluster share the
+  // weight slices (the N2NMN_EXP_PROJ_PAIRS build of proj_wgmma.cuh). The two tiles share only
+  // the weight matrix, so a tile is paired with the next tile of its layer wherever that one comes
+  // from. A layer with an odd tile count gets a filler half (pass = -1: skipped by the single-CTA
+  // kernel; the cluster form runs the MMA on the repeated tile and writes nothing).
   const int seg_rows = images_per_seg * HW;
   const int tiles_per_seg = (seg_rows + 127) / 128;
   S.work.reserve((size_t)tiles_per_seg * std::max(1, S.num_seg));

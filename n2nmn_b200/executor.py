@@ -294,7 +294,7 @@ class ExecutorPool:
     fill the SMs on its own; successive batches are independent (eval). submit() only queues the
     batch; each context's C++ worker thread (csrc/pool.cpp) takes up to `max_group` queued batches
     at a time and runs them with ONE set of launches (n2nmn_forward_group), so the contraction
-    kernel's CTA pairs walk several tiles each and the kernels of different contexts overlap on
+    kernel's persistent CTAs walk several tiles each and the kernels of different contexts overlap on
     the GPU. Each executor owns its workspaces, so there is no sharing hazard; weights are
     replicated (a few MB).
 
@@ -304,7 +304,7 @@ class ExecutorPool:
     def __init__(self, family, image_feat_grid, word_vecs, num_choices, assembler, weights=None,
                  num_streams=4, tree_cluster=None, proj_ctas=None, max_group=None, **ctx_kwargs):
         nb = int(ctx_kwargs.get('max_batch') or image_feat_grid.shape[0])
-        if max_group is None:   # ~1024 questions per launch set: the contraction kernel's CTA pairs
+        if max_group is None:   # ~1024 questions per launch set: the contraction kernel's CTAs
             # then walk 10+ tiles each (0.49 of the TF32 peak against 0.42 at 512; 6.2 M vs 5.3 M q/s)
             max_group = 1 if num_streams == 1 else max(1, min(16, 1024 // max(nb, 1)))
         if 'N2NMN_MAX_GROUP' in os.environ:
@@ -320,8 +320,8 @@ class ExecutorPool:
         # Several batches in flight: throughput, not the latency of one batch, is what counts. The
         # node kernels of a batch are latency chains, so the GPU does more work per second with
         # one CTA per question and many questions per launch than with a question spread over a
-        # cluster (measured: DESIGN §9). The contraction kernel keeps the whole grid of CTA pairs:
-        # a group gives every pair several tiles.
+        # cluster (measured: DESIGN §9). The contraction kernel keeps its whole persistent grid:
+        # a group gives every CTA several tiles.
         if tree_cluster is None:
             tree_cluster = 0 if num_streams == 1 else 1
         if proj_ctas is None:

@@ -10,11 +10,13 @@
 #include <cmath>
 #include <cstring>
 #include <ctime>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/n2nmn_b200.h"
 #include "common.cuh"
+#include "launch.cuh"
 #include "node_eval.cuh"
 #include "prep.cuh"
 #include "proj_simt.cuh"
@@ -45,7 +47,26 @@ int fail(int code, const std::string& msg) {
       return fail(N2NMN_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));   \
   } while (0)
 
+#define TRY(expr)                                                                       \
+  do {                                                                                  \
+    if (int _rc = (expr)) return _rc;                                                   \
+  } while (0)
+
+// Lazy workspaces allocate through this, so that a retry after a failed setup allocates only what
+// is still missing.
+template <class T>
+cudaError_t alloc_once(T** p, size_t bytes) {
+  return *p ? cudaSuccess : cudaMalloc(p, bytes);
+}
+
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+
+// VQA features gain two coordinate channels and its Transform has no filter bank
+SchedShape sched_shape(const n2nmn_config& g) {
+  const bool vqa = g.family == N2NMN_VQA;
+  return SchedShape{g.family, g.H, g.W, g.D + (vqa ? 2 : 0), g.text_dim, g.map_dim,
+                    round_up(g.map_dim, 256), g.num_choices, vqa ? 1 : g.kernel_size, g.max_T};
+}
 
 enum VarKind { VK_PLAIN = 0, VK_PROJ_W, VK_PROJ_B, VK_PITCHED };
 
@@ -74,6 +95,20 @@ struct TableOffsets {
       wave_nodes, bwd_nodes, entry_order, node_entry, entries, text_set_start, labels, head_work, head_list, pool_img,
       total;
 };
+
+// Calls f(offset field, host bytes, byte count) for every schedule table, in device order. The
+// labels of a training schedule come from the caller (`labels`, may be null), not from S.
+template <class O, class F>
+void for_each_table(const HostSchedule& S, const int32_t* labels, O& o, F&& f) {
+  auto v = [&](auto& off, const auto& vec) { f(off, vec.data(), vec.size() * sizeof(vec[0])); };
+  v(o.nodes, S.nodes); v(o.q_ptr, S.q_ptr); v(o.text_t, S.text_t); v(o.text_b, S.text_b);
+  v(o.groups, S.groups); v(o.work, S.work); v(o.img_ptr, S.img_ptr); v(o.node_text, S.node_text);
+  v(o.node_out, S.node_out); v(o.mslot, S.mslot); v(o.wave_nodes, S.wave_nodes);
+  v(o.bwd_nodes, S.bwd_nodes); v(o.entry_order, S.entry_order); v(o.node_entry, S.node_entry);
+  v(o.entries, S.entries); v(o.text_set_start, S.text_set_start);
+  f(o.labels, labels, S.train ? (S.q_ptr.size() - 1) * 4 : 0);
+  v(o.head_work, S.head_work); v(o.head_list, S.head_list); v(o.pool_img, S.pool_img);
+}
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                   const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -135,7 +170,8 @@ struct n2nmn_ctx {
   bool use_pdl = true;         // programmatic dependent launch between the three kernels
   n2nmn_sched module_sched;    // scratch schedule of n2nmn_module_fwd
   n2nmn_sched step_sched;      // scratch schedule of n2nmn_forward_tokens
-  // training workspaces (allocated on first use)
+  // training workspaces (allocated on first use; ready once every allocation and attribute is set)
+  bool train_ready = false;
   const int32_t* train_labels = nullptr;   // host labels of the step being compiled
   const uint8_t* last_tables = nullptr;    // device tables of the last run_tables
   TableOffsets last_offsets;
@@ -169,9 +205,11 @@ struct n2nmn_ctx {
   HeadTailMaps ht_maps[NUM_OUT_SETS];
   int Cpad = 0;   // [max_batch][HW][Mp] scratch of the Transform backward
   int dmap_entries = 0;
-  VarSeg* d_segs = nullptr;
+  VarSeg* d_segs = nullptr;                // Adam segment table, ready with d_sumsq
   float* d_sumsq = nullptr;
+  bool segs_ready = false;
   RepackSeg* d_repack = nullptr;           // fused re-pack tables (n2nmn_load_flat_weights)
+  bool repack_ready = false;
   ProjRepack proj_repack;
   int proj_repack_sets = 0;
   float dword_scale = 1.f;                 // n2nmn_set_grad_scale
@@ -291,35 +329,21 @@ int encode_2d(n2nmn_ctx* c, CUtensorMap* map, const float* base, uint64_t inner,
 TableOffsets table_offsets(const HostSchedule& S) {
   TableOffsets o;
   size_t off = 0;
-  auto take = [&](size_t bytes) { size_t at = off; off += (bytes + 15) & ~(size_t)15; return at; };
-  o.nodes = take(S.nodes.size() * sizeof(NodeRec));
-  o.q_ptr = take(S.q_ptr.size() * 4);
-  o.text_t = take(S.text_t.size() * 4);
-  o.text_b = take(S.text_b.size() * 4);
-  o.groups = take(S.groups.size() * sizeof(TextGroup));
-  o.work = take(S.work.size() * sizeof(ProjWork));
-  o.img_ptr = take(S.img_ptr.size() * 4);
-  o.node_text = take(S.node_text.size() * 4);
-  o.node_out = take(S.node_out.size() * 4);
-  o.mslot = take(S.mslot.size() * 4);
-  o.wave_nodes = take(S.wave_nodes.size() * 4);
-  o.bwd_nodes = take(S.bwd_nodes.size() * 4);
-  o.entry_order = take(S.entry_order.size() * 4);
-  o.node_entry = take(S.node_entry.size() * 4);
-  o.entries = take(S.entries.size() * sizeof(BwdEntryHost));
-  o.text_set_start = take(S.text_set_start.size() * 4);
-  o.labels = take(S.train ? (S.q_ptr.size() - 1) * 4 : 0);
-  o.head_work = take(S.head_work.size() * sizeof(HeadWork));
-  o.head_list = take(S.head_list.size() * 4);
-  o.pool_img = take(S.pool_img.size() * 4);
+  for_each_table(S, nullptr, o, [&](size_t& at, const void*, size_t bytes) {
+    at = off;
+    off += (bytes + 15) & ~(size_t)15;
+  });
   o.total = off;
   return o;
 }
 
-template <class V>
-void put(uint8_t* base, size_t off, const V& v) {
-  if (!v.empty()) std::memcpy(base + off, v.data(), v.size() * sizeof(v[0]));
-}
+// The device copy of a schedule's tables.
+struct DevTables {
+  const uint8_t* d;
+  TableOffsets o;
+  template <class T = int32_t>
+  const T* at(size_t off) const { return reinterpret_cast<const T*>(d + off); }
+};
 
 void prof_mark(n2nmn_ctx* c, const char* name, cudaStream_t st) {
   if (!c->profiling) return;
@@ -331,6 +355,239 @@ void prof_mark(n2nmn_ctx* c, const char* name, cudaStream_t st) {
   }
   c->ev_names[c->ev_used] = name;
   cudaEventRecord(c->ev[c->ev_used++], st);
+}
+
+// Every kernel launch of the context goes through here and is counted once.
+template <class... KArgs, class... Args>
+int ctx_launch(n2nmn_ctx* c, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
+               cudaStream_t st, LaunchAttrs a, Args... args) {
+  const cudaError_t e = launch(kernel, grid, block, smem, st, a, args...);
+  if (e != cudaSuccess) return fail(N2NMN_ERR_CUDA, std::string("kernel launch: ") + cudaGetErrorString(e));
+  ++c->launches;
+  return 0;
+}
+
+// Maximum dynamic shared memory of a kernel and, if carveout >= 0, its preferred carveout.
+template <class... KArgs>
+int set_smem(void (*kernel)(KArgs...), int bytes, int carveout = -1) {
+  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  if (carveout >= 0)
+    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
+  return 0;
+}
+
+// Kernel variants, chosen in one place for the attribute setup and the launch.
+auto tree_variant(int ks, bool direct) {
+  if (direct) return ks == 5 ? &tree_kernel<5, true> : &tree_kernel<3, true>;
+  return ks == 5 ? &tree_kernel<5, false> : &tree_kernel<3, false>;
+}
+auto wave_variant(int ks) { return ks == 5 ? &wave_kernel<5> : &wave_kernel<3>; }
+auto head_variant(int nn) {
+  return nn == 16 ? &head_kernel<16> : nn == 8 ? &head_kernel<8> : &head_kernel<4>;
+}
+auto tail_gemm_variant(bool narrow) {
+  return narrow ? &head_tail_gemm_kernel<2> : &head_tail_gemm_kernel<4>;
+}
+// VQA walks Find-type nodes only (in two channel passes when wide); the conv families run the
+// Transform instantiation on a level with Transform nodes (tr) and the lighter one otherwise
+auto bwd_variant(bool vqa, bool tr, int ks, bool wide) {
+  if (vqa) return wide ? &tree_bwd_kernel<1, false, true> : &tree_bwd_kernel<1, false, false>;
+  if (tr) return ks == 5 ? &tree_bwd_kernel<5, true> : &tree_bwd_kernel<3, true>;
+  return ks == 5 ? &tree_bwd_kernel<5, false> : &tree_bwd_kernel<3, false>;
+}
+
+// Makes the schedule's tables resident in a table slot, uploading them unless a slot holds them.
+int upload_tables(n2nmn_ctx* c, const n2nmn_sched* sc, const TableOffsets& o, cudaStream_t st,
+                  TableSlot** out) {
+  for (int i = 0; i < kTableSlots; ++i)
+    if (c->slots[i].uid == sc->uid) *out = &c->slots[i];
+  if (*out) return 0;
+  TableSlot* slot = *out = &c->slots[c->next_slot];
+  c->next_slot = (c->next_slot + 1) % kTableSlots;
+  CUDA_TRY(cudaEventSynchronize(slot->last_use));   // previous tenant no longer in flight
+  for_each_table(sc->hs, c->train_labels, o, [&](size_t at, const void* src, size_t bytes) {
+    if (src && bytes) std::memcpy(slot->host + at, src, bytes);
+  });
+  CUDA_TRY(cudaMemcpyAsync(slot->dev, slot->host, o.total, cudaMemcpyHostToDevice, st));
+  slot->uid = sc->uid;
+  return 0;
+}
+
+// K1: text projections (+ the quadratic-form coefficients of the Transform nodes)
+int text_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, cudaStream_t st) {
+  if (S.groups.empty()) return 0;
+  TextSetRows tsr;
+  for (int i = 0; i <= NUM_TEXT_SETS; ++i) tsr.start[i] = S.text_set_start[i];
+  TRY(ctx_launch(c, text_proj_kernel, dim3((unsigned)(c->Mp / kMmaCols), (unsigned)S.groups.size()),
+                 kMmaThreads, mma_smem_bytes(4, kTextStages), st, {}, c->md, c->tb, tsr,
+                 t.at(t.o.text_t), t.at(t.o.text_b)));
+  prof_mark(c, "text_proj_kernel", st);
+  const int tr0 = S.text_set_start[TS_TRANSFORM];
+  const int trn = S.text_set_start[TS_TRANSFORM + 1] - tr0;
+  if (trn > 0 && c->conv_quad) {
+    const int qcols = quad_pitch(c->cfg.kernel_size) - quad_u_pitch(c->cfg.kernel_size);
+    TRY(ctx_launch(c, quad_kernel,
+                   dim3((unsigned)(1 + (qcols + kMmaCols - 1) / kMmaCols), (unsigned)((trn + 63) / 64)),
+                   kMmaThreads, mma_smem_bytes(4, kTextStages), st, {c->use_pdl}, c->md, c->tb,
+                   tr0, trn));
+    prof_mark(c, "quad_kernel", st);
+  }
+  return 0;
+}
+
+// K2: conv_image contraction with fused Find / stored FindSameProperty maps
+int contraction_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, float* arena,
+                      cudaStream_t st) {
+  if (S.work.empty()) return 0;
+  ProjParams p;
+  p.work = t.at<ProjWork>(t.o.work);
+  p.num_work = (int)S.work.size();
+  p.total_rows = c->md.N * c->HW;
+  p.num_seg = c->md.num_seg;
+  p.seg_images = c->md.N;
+  p.n_tiles = c->Mp / 256;
+  p.k_blocks = (c->Dk + kBK - 1) / kBK;
+  p.HW = c->HW; p.M = c->cfg.map_dim; p.Mp = c->Mp; p.Dk = c->Dk;
+  p.feat_pitch = c->md.feat_pitch;
+  for (int s = 0; s < kMaxSeg; ++s) p.feat_seg[s] = c->md.feat_seg[s];
+  for (int s = 0; s < NUM_PROJ_SETS; ++s) {
+    p.bias[s] = c->proj_bias[s];
+    p.w_orig[s] = c->md.proj_w[s];
+  }
+  p.img_ptr = t.at(t.o.img_ptr);
+  p.node_text = t.at(t.o.node_text);
+  p.node_out = t.at(t.o.node_out);
+  p.tauw = c->tb.tauw; p.tau2 = c->tb.tau2;
+  p.elt_b = c->md.elt_b[ES_FIND];
+  p.arena = arena;
+  p.mslot = t.at(t.o.mslot);
+  p.num_images = (int)(S.mslot.size() / NUM_PROJ_SETS);
+  p.mbuf = c->mbuf;
+  // persistent grid: CTA i walks the tiles i, i + CTAs, ... (two tiles per work item)
+  const int max_ctas = c->proj_max_ctas > 0 ? std::min(c->proj_max_ctas, c->num_sms) : c->num_sms;
+#if defined(N2NMN_EXP_PROJ_PAIRS)
+  // experiment build (proj_wgmma.cuh): an even grid of 2-CTA clusters, at most what fits at once
+  constexpr unsigned cluster = 2;
+  static int max_pairs = 0;
+  if (max_pairs == 0) {
+    cudaLaunchConfig_t oc;
+    std::memset(&oc, 0, sizeof(oc));
+    oc.gridDim = dim3((unsigned)(2 * (c->num_sms / 2)));
+    oc.blockDim = dim3(kProjThreads);
+    oc.dynamicSmemBytes = proj_smem_bytes();
+    cudaLaunchAttribute ca[1];
+    ca[0].id = cudaLaunchAttributeClusterDimension;
+    ca[0].val.clusterDim.x = 2; ca[0].val.clusterDim.y = 1; ca[0].val.clusterDim.z = 1;
+    oc.attrs = ca;
+    oc.numAttrs = 1;
+    CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, proj_wgmma_kernel, &oc));
+    if (max_pairs < 1) return fail(N2NMN_ERR_CUDA, "no 2-CTA cluster of the projection kernel fits");
+  }
+  const int ctas = 2 * std::max(1, std::min({p.num_work, max_ctas / 2, max_pairs}));
+#else
+  constexpr unsigned cluster = 1;
+  const int ctas = std::max(1, std::min(2 * p.num_work, max_ctas));
+#endif
+  if (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) {
+    const size_t smem = (size_t)(kSimtRows * kSimtKChunk + kSimtRows * c->Mp) * sizeof(float);
+    TRY(ctx_launch(c, proj_simt_kernel, 2 * p.num_work, 256, smem, st, {}, p));
+    prof_mark(c, "proj_simt_kernel", st);
+  } else {
+    TRY(ctx_launch(c, proj_wgmma_kernel, ctas, kProjThreads, proj_smem_bytes(), st,
+                   {c->use_pdl, cluster}, c->tmaps, p));
+    prof_mark(c, "proj_wgmma_kernel", st);
+  }
+  return 0;
+}
+
+// K3: node evaluation, by depth waves or one tree walk per question
+int node_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, const NodeCtx& nc,
+               float* const* scores_seg, bool use_wave, bool write_arena, cudaStream_t st) {
+  const int NQ = (int)S.q_ptr.size() - 1;
+  const int nseg = std::max(1, S.num_seg);
+  const int ks = c->cfg.kernel_size;
+  const NodeRec* d_nodes = t.at<NodeRec>(t.o.nodes);
+  if (use_wave) {
+    for (int s = 0; s < nseg; ++s)
+      CUDA_TRY(cudaMemsetAsync(scores_seg[s], 0,
+                               (size_t)(nseg > 1 ? S.N : NQ) * c->cfg.num_choices * sizeof(float),
+                               st));
+    for (int dep = 1; dep <= S.max_depth; ++dep) {
+      const int first = S.wave_ptr[dep], cnt = S.wave_ptr[dep + 1] - first;
+      if (cnt == 0) continue;
+      TRY(ctx_launch(c, wave_variant(ks), cnt, kNodeThreads, c->node_smem_bytes, st, {}, nc,
+                     d_nodes, t.at(t.o.wave_nodes), first));
+      prof_mark(c, "wave_kernel", st);
+    }
+    return 0;
+  }
+  if (NQ <= 0) return 0;
+  // cluster size: spread one question over several SMs while the batch is small
+  int cs = c->tree_cluster;
+  if (cs <= 0) cs = (NQ * 4 <= 2 * c->num_sms) ? 4 : (NQ * 2 <= 2 * c->num_sms) ? 2 : 1;
+  const int slots = std::max(1, S.max_stack);
+  const size_t smem = sizeof(float) * (size_t)tree_smem_layout(
+      c->cfg.H, c->cfg.W, c->Mp, ks, c->cfg.map_dim, c->cfg.num_choices, slots,
+      S.pooled_direct).total;
+  const int wa = (write_arena ? kTreeWriteArena : 0) |
+                 (((c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) || c->fp32_stencil) ? kTreeFp32Stencil : 0);
+  TRY(ctx_launch(c, tree_variant(ks, S.pooled_direct), NQ * cs, kNodeThreads, smem, st,
+                 {c->use_pdl, (unsigned)cs}, nc, d_nodes, t.at(t.o.q_ptr), cs, slots, wa));
+  prof_mark(c, "tree_kernel", st);
+  return 0;
+}
+
+// K4: batched answer heads of the attention-pooled roots of the tree executor
+int head_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, const NodeCtx& nc,
+               cudaStream_t st) {
+  if (!S.pooled_direct || S.head_work.empty()) return 0;
+  if ((int)S.num_pool_rows > 2 * c->QB)
+    return fail(N2NMN_ERR_CAPACITY, "too many pooled root nodes for this context");
+  const LaunchAttrs pdl{c->use_pdl};
+  if (S.num_feat_rows > 0) {   // pooled features: one CTA per (root row, 128-channel chunk)
+    const int HWp = (c->HW + 3) & ~3;
+    const int quads = c->md.feat_pitch / 4;
+    TRY(ctx_launch(c, pool_kernel,
+                   dim3((unsigned)S.num_feat_rows, (unsigned)((quads + kPoolQuads - 1) / kPoolQuads)),
+                   kPoolQuads * kPoolSlices, (size_t)(HWp + 4 * kPoolQuads * kPoolSlices) * sizeof(float),
+                   st, pdl, nc, t.at(t.o.pool_img), HWp));
+    prof_mark(c, "pool_kernel", st);
+  }
+  TRY(ctx_launch(c, head_variant(c->head_nn), (unsigned)S.head_work.size(), kHeadThreads,
+                 (size_t)c->head_smem_bytes, st, pdl, nc, t.at<NodeRec>(t.o.nodes),
+                 t.at<HeadWork>(t.o.head_work), t.at(t.o.head_list)));
+  prof_mark(c, "head_kernel", st);
+  if (!c->ehat) return 0;
+  // fc_eltwise of the Describe-type roots as one GEMM per weight set
+  const bool tail_wgmma = c->ehat_lo && !std::getenv("N2NMN_TAIL_MMA_SYNC");
+  for (int op : {OP_DESCRIBE, OP_SAME_PROPERTY}) {
+    int r0 = 1 << 30, r1 = 0;
+    for (const HeadWork& w : S.head_work)
+      if (w.op == op) { r0 = std::min(r0, (int)w.first); r1 = std::max(r1, (int)(w.first + w.count)); }
+    if (r1 <= r0) continue;
+    const int os = op == OP_DESCRIBE ? OS_DESCRIBE : OS_SAMEPROP;
+    if (!c->out_wp[os]) return fail(N2NMN_ERR_STATE, "answer-head weights not packed");
+    if (tail_wgmma && c->out_wt_hi[os]) {
+      TRY(ctx_launch(c, head_tail_wgmma_kernel,
+                     dim3((unsigned)(c->Cpad / kHtN), (unsigned)((r1 - r0 + kHtM - 1) / kHtM)),
+                     kHtThreads, kHtSmemBytes, st, pdl, c->ht_maps[os], c->md.out_b[os],
+                     (float* const*)c->ehat_dst, r0, r1 - r0, (int)c->cfg.num_choices,
+                     (int)c->cfg.map_dim));
+    } else {
+      GemmOperands gp;
+      gp.a0 = c->ehat + (size_t)r0 * c->Mp; gp.k0 = c->cfg.map_dim; gp.lda0 = c->Mp;
+      gp.a1 = nullptr; gp.k1 = 0; gp.lda1 = 0;
+      gp.R = r1 - r0; gp.B = c->out_wp[os]; gp.ldb = c->Cp; gp.C = c->cfg.num_choices;
+      const bool narrow = gp.R <= 32;
+      TRY(ctx_launch(c, tail_gemm_variant(narrow),
+                     dim3((unsigned)((gp.C + kMmaCols - 1) / kMmaCols),
+                          (unsigned)(narrow ? (gp.R + 31) / 32 : (gp.R + 63) / 64)),
+                     kMmaThreads, mma_smem_bytes(narrow ? 2 : 4), st, pdl, gp, c->md.out_b[os],
+                     (float* const*)c->ehat_dst, r0));
+    }
+    prof_mark(c, "head_tail_gemm_kernel", st);
+  }
+  return 0;
 }
 
 // Uploads (if needed) and launches everything for one compiled batch.
@@ -355,303 +612,54 @@ int run_tables(n2nmn_ctx* c, n2nmn_sched* sc, float* const* scores_seg, float* a
     return fail(N2NMN_ERR_CAPACITY, "too many text nodes for this context");
   if (S.num_mslots > c->mbuf_slots)
     return fail(N2NMN_ERR_CAPACITY, "too many stored feature maps for this context");
-  // ---- table residency
   TableSlot* slot = nullptr;
-  for (int i = 0; i < kTableSlots; ++i)
-    if (c->slots[i].uid == sc->uid) slot = &c->slots[i];
-  if (!slot) {
-    slot = &c->slots[c->next_slot];
-    c->next_slot = (c->next_slot + 1) % kTableSlots;
-    CUDA_TRY(cudaEventSynchronize(slot->last_use));   // previous tenant no longer in flight
-    put(slot->host, o.nodes, S.nodes);
-    put(slot->host, o.q_ptr, S.q_ptr);
-    put(slot->host, o.text_t, S.text_t);
-    put(slot->host, o.text_b, S.text_b);
-    put(slot->host, o.groups, S.groups);
-    put(slot->host, o.work, S.work);
-    put(slot->host, o.img_ptr, S.img_ptr);
-    put(slot->host, o.node_text, S.node_text);
-    put(slot->host, o.node_out, S.node_out);
-    put(slot->host, o.mslot, S.mslot);
-    put(slot->host, o.wave_nodes, S.wave_nodes);
-    put(slot->host, o.bwd_nodes, S.bwd_nodes);
-    put(slot->host, o.entry_order, S.entry_order);
-    put(slot->host, o.node_entry, S.node_entry);
-    put(slot->host, o.entries, S.entries);
-    put(slot->host, o.text_set_start, S.text_set_start);
-    put(slot->host, o.head_work, S.head_work);
-    put(slot->host, o.head_list, S.head_list);
-    put(slot->host, o.pool_img, S.pool_img);
-    if (S.train && c->train_labels)
-      std::memcpy(slot->host + o.labels, c->train_labels, (S.q_ptr.size() - 1) * 4);
-    CUDA_TRY(cudaMemcpyAsync(slot->dev, slot->host, o.total, cudaMemcpyHostToDevice, st));
-    slot->uid = sc->uid;
-  }
-  const uint8_t* d = slot->dev;
-  c->last_tables = d;
+  TRY(upload_tables(c, sc, o, st, &slot));
+  const DevTables t{slot->dev, o};
+  c->last_tables = slot->dev;
   c->last_offsets = o;
-  const NodeRec* d_nodes = reinterpret_cast<const NodeRec*>(d + o.nodes);
-  const int32_t* d_qptr = reinterpret_cast<const int32_t*>(d + o.q_ptr);
 
-  c->ev_used = 0;
-  prof_mark(c, "begin", st);
-  // every kernel of the step after the first is a programmatic dependent launch of its
-  // predecessor (each calls griddepcontrol.wait before it touches the predecessor's output)
-  auto pdl_ok = [&]() { return c->use_pdl; };
-  // ---- K1 text projections (+ the quadratic-form coefficients of the Transform nodes)
-  if (!S.groups.empty()) {
-    dim3 grid((unsigned)(c->Mp / kMmaCols), (unsigned)S.groups.size());
-    TextSetRows tsr;
-    for (int i = 0; i <= NUM_TEXT_SETS; ++i) tsr.start[i] = S.text_set_start[i];
-    text_proj_kernel<<<grid, kMmaThreads, mma_smem_bytes(4, kTextStages), st>>>(
-        c->md, c->tb, tsr,
-        reinterpret_cast<const int32_t*>(d + o.text_t),
-        reinterpret_cast<const int32_t*>(d + o.text_b));
-    ++c->launches;
-    prof_mark(c, "text_proj_kernel", st);
-    const int tr0 = S.text_set_start[TS_TRANSFORM];
-    const int trn = S.text_set_start[TS_TRANSFORM + 1] - tr0;
-    if (trn > 0 && c->conv_quad) {
-      cudaLaunchConfig_t qc;
-      std::memset(&qc, 0, sizeof(qc));
-      const int qcols = quad_pitch(c->cfg.kernel_size) - quad_u_pitch(c->cfg.kernel_size);
-      qc.gridDim = dim3((unsigned)(1 + (qcols + kMmaCols - 1) / kMmaCols), (unsigned)((trn + 63) / 64));
-      qc.blockDim = dim3(kMmaThreads);
-      qc.dynamicSmemBytes = mma_smem_bytes(4, kTextStages);
-      qc.stream = st;
-      cudaLaunchAttribute qa[1];
-      qa[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      qa[0].val.programmaticStreamSerializationAllowed = 1;
-      qc.attrs = qa;
-      qc.numAttrs = pdl_ok() ? 1 : 0;
-      CUDA_TRY(cudaLaunchKernelEx(&qc, quad_kernel, c->md, c->tb, tr0, trn));
-      ++c->launches;
-      prof_mark(c, "quad_kernel", st);
-    }
-  }
-  // ---- K2 conv_image contraction with fused Find / stored FindSameProperty maps
-  if (!S.work.empty()) {
-    ProjParams p;
-    p.work = reinterpret_cast<const ProjWork*>(d + o.work);
-    p.num_work = (int)S.work.size();
-    p.total_rows = c->md.N * c->HW;
-    p.num_seg = c->md.num_seg;
-    p.seg_images = c->md.N;
-    p.n_tiles = c->Mp / 256;
-    p.k_blocks = (c->Dk + kBK - 1) / kBK;
-    p.HW = c->HW; p.M = c->cfg.map_dim; p.Mp = c->Mp; p.Dk = c->Dk;
-    p.feat_pitch = c->md.feat_pitch;
-    for (int s = 0; s < kMaxSeg; ++s) p.feat_seg[s] = c->md.feat_seg[s];
-    for (int s = 0; s < NUM_PROJ_SETS; ++s) {
-      p.bias[s] = c->proj_bias[s];
-      p.w_orig[s] = c->md.proj_w[s];
-    }
-    p.img_ptr = reinterpret_cast<const int32_t*>(d + o.img_ptr);
-    p.node_text = reinterpret_cast<const int32_t*>(d + o.node_text);
-    p.node_out = reinterpret_cast<const int32_t*>(d + o.node_out);
-    p.tauw = c->tb.tauw; p.tau2 = c->tb.tau2;
-    p.elt_b = c->md.elt_b[ES_FIND];
-    p.arena = arena;
-    p.mslot = reinterpret_cast<const int32_t*>(d + o.mslot);
-    p.num_images = (int)(S.mslot.size() / NUM_PROJ_SETS);
-    p.mbuf = c->mbuf;
-    // persistent grid: CTA i walks the tiles i, i + CTAs, ... (two tiles per work item)
-    const int max_ctas = c->proj_max_ctas > 0 ? std::min(c->proj_max_ctas, c->num_sms) : c->num_sms;
-#if defined(N2NMN_EXP_PROJ_PAIRS)
-    // experiment build (proj_wgmma.cuh): an even grid of 2-CTA clusters, at most what fits at once
-    static int max_pairs = 0;
-    if (max_pairs == 0) {
-      cudaLaunchConfig_t oc;
-      std::memset(&oc, 0, sizeof(oc));
-      oc.gridDim = dim3((unsigned)(2 * (c->num_sms / 2)));
-      oc.blockDim = dim3(kProjThreads);
-      oc.dynamicSmemBytes = proj_smem_bytes();
-      cudaLaunchAttribute ca[1];
-      ca[0].id = cudaLaunchAttributeClusterDimension;
-      ca[0].val.clusterDim.x = 2; ca[0].val.clusterDim.y = 1; ca[0].val.clusterDim.z = 1;
-      oc.attrs = ca;
-      oc.numAttrs = 1;
-      CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, proj_wgmma_kernel, &oc));
-      if (max_pairs < 1) return fail(N2NMN_ERR_CUDA, "no 2-CTA cluster of the projection kernel fits");
-    }
-    const int ctas = 2 * std::max(1, std::min({p.num_work, max_ctas / 2, max_pairs}));
-#else
-    const int ctas = std::max(1, std::min(2 * p.num_work, max_ctas));
-#endif
-    if (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) {
-      const size_t smem = (size_t)(kSimtRows * kSimtKChunk + kSimtRows * c->Mp) * sizeof(float);
-      proj_simt_kernel<<<2 * p.num_work, 256, smem, st>>>(p);
-      prof_mark(c, "proj_simt_kernel", st);
-    } else {
-      cudaLaunchConfig_t lc;
-      std::memset(&lc, 0, sizeof(lc));
-      lc.gridDim = dim3((unsigned)ctas);
-      lc.blockDim = dim3(kProjThreads);
-      lc.dynamicSmemBytes = proj_smem_bytes();
-      lc.stream = st;
-      cudaLaunchAttribute attr[2];
-      int na = 0;
-#if defined(N2NMN_EXP_PROJ_PAIRS)
-      attr[na].id = cudaLaunchAttributeClusterDimension;
-      attr[na].val.clusterDim.x = 2; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-      ++na;
-#endif
-      if (pdl_ok()) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-      }
-      lc.attrs = attr;
-      lc.numAttrs = na;
-      CUDA_TRY(cudaLaunchKernelEx(&lc, proj_wgmma_kernel, c->tmaps, p));
-      prof_mark(c, "proj_wgmma_kernel", st);
-    }
-    ++c->launches;
-  }
-  // ---- K3 node evaluation
   NodeCtx nc;
   nc.md = c->md; nc.tb = c->tb; nc.arena = arena; nc.scores = scores_seg[0]; nc.mbuf = c->mbuf;
   nc.pooled = c->pooled; nc.pool_pitch = c->Kp; nc.pool_att = c->pool_att;
   nc.phi_out = S.train ? c->phi_buf : nullptr;
   nc.ehat = c->ehat; nc.ehat_lo = c->ehat_lo; nc.ehat_dst = c->ehat_dst;
-  const int NQ = (int)S.q_ptr.size() - 1;
   // several segments: question q writes row q % N of segment q / N; one segment: row q (the
   // per-module entry point numbers its call rows beyond the bound batch size)
   const int nseg = std::max(1, S.num_seg);
   nc.score_rows = nseg > 1 ? S.N : (1 << 30);
   for (int s = 0; s < kMaxSeg; ++s) nc.scores_seg[s] = scores_seg[s < nseg ? s : 0];
-  const bool ks3 = (c->cfg.kernel_size != 5);
-  if (use_wave) {
-    for (int s = 0; s < nseg; ++s)
-      CUDA_TRY(cudaMemsetAsync(scores_seg[s], 0,
-                               (size_t)(nseg > 1 ? S.N : NQ) * c->cfg.num_choices * sizeof(float),
-                               st));
-    const int32_t* d_wave = reinterpret_cast<const int32_t*>(d + o.wave_nodes);
-    for (int dep = 1; dep <= S.max_depth; ++dep) {
-      const int first = S.wave_ptr[dep], cnt = S.wave_ptr[dep + 1] - first;
-      if (cnt == 0) continue;
-      if (ks3) wave_kernel<3><<<cnt, kNodeThreads, c->node_smem_bytes, st>>>(nc, d_nodes, d_wave, first);
-      else wave_kernel<5><<<cnt, kNodeThreads, c->node_smem_bytes, st>>>(nc, d_nodes, d_wave, first);
-      ++c->launches;
-      prof_mark(c, "wave_kernel", st);
-    }
-  } else if (NQ > 0) {
-    // cluster size: spread one question over several SMs while the batch is small
-    int cs = c->tree_cluster;
-    if (cs <= 0) cs = (NQ * 4 <= 2 * c->num_sms) ? 4 : (NQ * 2 <= 2 * c->num_sms) ? 2 : 1;
-    cudaLaunchConfig_t lc;
-    std::memset(&lc, 0, sizeof(lc));
-    lc.gridDim = dim3((unsigned)(NQ * cs));
-    lc.blockDim = dim3(kNodeThreads);
-    const int slots = std::max(1, S.max_stack);
-    lc.dynamicSmemBytes = sizeof(float) * (size_t)tree_smem_layout(
-        c->cfg.H, c->cfg.W, c->Mp, c->cfg.kernel_size, c->cfg.map_dim, c->cfg.num_choices,
-        slots, S.pooled_direct).total;
-    lc.stream = st;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (cs > 1) {
-      attr[na].id = cudaLaunchAttributeClusterDimension;
-      attr[na].val.clusterDim.x = (unsigned)cs;
-      attr[na].val.clusterDim.y = 1;
-      attr[na].val.clusterDim.z = 1;
-      ++na;
-    }
-    if (pdl_ok()) {
-      attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[na].val.programmaticStreamSerializationAllowed = 1;
-      ++na;
-    }
-    lc.attrs = attr;
-    lc.numAttrs = na;
-    const int wa = (write_arena ? kTreeWriteArena : 0) |
-                   (((c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) || c->fp32_stencil) ? kTreeFp32Stencil : 0);
-    if (S.pooled_direct) {
-      if (ks3) CUDA_TRY(cudaLaunchKernelEx(&lc, tree_kernel<3, true>, nc, d_nodes, d_qptr, cs, slots, wa));
-      else CUDA_TRY(cudaLaunchKernelEx(&lc, tree_kernel<5, true>, nc, d_nodes, d_qptr, cs, slots, wa));
-    } else {
-      if (ks3) CUDA_TRY(cudaLaunchKernelEx(&lc, tree_kernel<3, false>, nc, d_nodes, d_qptr, cs, slots, wa));
-      else CUDA_TRY(cudaLaunchKernelEx(&lc, tree_kernel<5, false>, nc, d_nodes, d_qptr, cs, slots, wa));
-    }
-    ++c->launches;
-    prof_mark(c, "tree_kernel", st);
-    // ---- K4 batched answer heads of the attention-pooled roots
-    if (S.pooled_direct && !S.head_work.empty()) {
-      if ((int)S.num_pool_rows > 2 * c->QB)
-        return fail(N2NMN_ERR_CAPACITY, "too many pooled root nodes for this context");
-      cudaLaunchConfig_t hc;
-      std::memset(&hc, 0, sizeof(hc));
-      hc.gridDim = dim3((unsigned)S.head_work.size());
-      hc.blockDim = dim3(kHeadThreads);
-      hc.dynamicSmemBytes = (size_t)c->head_smem_bytes;
-      hc.stream = st;
-      cudaLaunchAttribute hattr[1];
-      hattr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      hattr[0].val.programmaticStreamSerializationAllowed = 1;
-      hc.attrs = hattr;
-      hc.numAttrs = pdl_ok() ? 1 : 0;
-      if (S.num_feat_rows > 0) {   // pooled features: one CTA per (root row, 128-channel chunk)
-        const int HWp = (c->HW + 3) & ~3;
-        cudaLaunchConfig_t pc = hc;
-        const int quads = c->md.feat_pitch / 4;
-        pc.gridDim = dim3((unsigned)S.num_feat_rows, (unsigned)((quads + kPoolQuads - 1) / kPoolQuads));
-        pc.blockDim = dim3(kPoolQuads * kPoolSlices);
-        pc.dynamicSmemBytes = (size_t)(HWp + 4 * kPoolQuads * kPoolSlices) * sizeof(float);
-        CUDA_TRY(cudaLaunchKernelEx(&pc, pool_kernel, nc,
-                                    reinterpret_cast<const int32_t*>(d + o.pool_img), HWp));
-        ++c->launches;
-        prof_mark(c, "pool_kernel", st);
-      }
-      const HeadWork* d_hw = reinterpret_cast<const HeadWork*>(d + o.head_work);
-      const int32_t* d_hl = reinterpret_cast<const int32_t*>(d + o.head_list);
-      if (c->head_nn == 16) CUDA_TRY(cudaLaunchKernelEx(&hc, head_kernel<16>, nc, d_nodes, d_hw, d_hl));
-      else if (c->head_nn == 8) CUDA_TRY(cudaLaunchKernelEx(&hc, head_kernel<8>, nc, d_nodes, d_hw, d_hl));
-      else CUDA_TRY(cudaLaunchKernelEx(&hc, head_kernel<4>, nc, d_nodes, d_hw, d_hl));
-      ++c->launches;
-      prof_mark(c, "head_kernel", st);
-      if (c->ehat) {   // fc_eltwise of the Describe-type roots as one GEMM per weight set
-        for (int op : {OP_DESCRIBE, OP_SAME_PROPERTY}) {
-          int r0 = 1 << 30, r1 = 0;
-          for (const HeadWork& w : S.head_work)
-            if (w.op == op) { r0 = std::min(r0, (int)w.first); r1 = std::max(r1, (int)(w.first + w.count)); }
-          if (r1 <= r0) continue;
-          const int os = op == OP_DESCRIBE ? OS_DESCRIBE : OS_SAMEPROP;
-          if (!c->out_wp[os]) return fail(N2NMN_ERR_STATE, "answer-head weights not packed");
-          if (c->ehat_lo && c->out_wt_hi[os] && !std::getenv("N2NMN_TAIL_MMA_SYNC")) {
-            cudaLaunchConfig_t tc = hc;
-            tc.gridDim = dim3((unsigned)(c->Cpad / kHtN), (unsigned)((r1 - r0 + kHtM - 1) / kHtM));
-            tc.blockDim = dim3(kHtThreads);
-            tc.dynamicSmemBytes = kHtSmemBytes;
-            CUDA_TRY(cudaLaunchKernelEx(&tc, head_tail_wgmma_kernel, c->ht_maps[os], c->md.out_b[os],
-                                        (float* const*)c->ehat_dst, r0, r1 - r0,
-                                        (int)c->cfg.num_choices, (int)c->cfg.map_dim));
-            ++c->launches;
-            prof_mark(c, "head_tail_gemm_kernel", st);
-            continue;
-          }
-          GemmOperands gp;
-          gp.a0 = c->ehat + (size_t)r0 * c->Mp; gp.k0 = c->cfg.map_dim; gp.lda0 = c->Mp;
-          gp.a1 = nullptr; gp.k1 = 0; gp.lda1 = 0;
-          gp.R = r1 - r0; gp.B = c->out_wp[os]; gp.ldb = c->Cp; gp.C = c->cfg.num_choices;
-          cudaLaunchConfig_t gc = hc;
-          const bool narrow = gp.R <= 32;
-          gc.gridDim = dim3((unsigned)((gp.C + kMmaCols - 1) / kMmaCols),
-                            (unsigned)(narrow ? (gp.R + 31) / 32 : (gp.R + 63) / 64));
-          gc.blockDim = dim3(kMmaThreads);
-          gc.dynamicSmemBytes = mma_smem_bytes(narrow ? 2 : 4);
-          if (narrow) CUDA_TRY(cudaLaunchKernelEx(&gc, head_tail_gemm_kernel<2>, gp, c->md.out_b[os],
-                                                  (float* const*)c->ehat_dst, r0));
-          else CUDA_TRY(cudaLaunchKernelEx(&gc, head_tail_gemm_kernel<4>, gp, c->md.out_b[os],
-                                           (float* const*)c->ehat_dst, r0));
-          ++c->launches;
-          prof_mark(c, "head_tail_gemm_kernel", st);
-        }
-      }
-    }
-  }
+
+  // every kernel of the step after the first is a programmatic dependent launch of its
+  // predecessor (each calls griddepcontrol.wait before it touches the predecessor's output)
+  c->ev_used = 0;
+  prof_mark(c, "begin", st);
+  TRY(text_stage(c, S, t, st));
+  TRY(contraction_stage(c, S, t, arena, st));
+  TRY(node_stage(c, S, t, nc, scores_seg, use_wave, write_arena, st));
+  TRY(head_stage(c, S, t, nc, st));
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaEventRecord(slot->last_use, st));
   return 0;
+}
+
+// The many-class answer tail's copies of fc_eltwise set `os` (row-pitched, and split into TF32
+// planes for wgmma), from its [map_dim, C] weights at `src`.
+int pack_out_weights(n2nmn_ctx* c, int os, const float* src, cudaStream_t st) {
+  if (!c->out_wp[os]) return 0;
+  TRY(ctx_launch(c, pitch_rows_kernel, c->cfg.map_dim, 256, 0, st, {}, src, c->cfg.map_dim,
+                 c->cfg.num_choices, c->out_wp[os], c->Cp));
+  if (c->out_wt_hi[os])
+    TRY(ctx_launch(c, out_wt_split_kernel, dim3((c->Cpad + 31) / 32, (c->Mp + 31) / 32), dim3(32, 8),
+                   0, st, {}, src, c->cfg.map_dim, c->cfg.num_choices, c->out_wt_hi[os],
+                   c->out_wt_lo[os], c->Mp, c->Cpad));
+  return 0;
+}
+
+int update_conv_quad(n2nmn_ctx* c, cudaStream_t st) {
+  if (!c->conv_quad) return 0;
+  return ctx_launch(c, conv_quad_kernel, quad_pitch(c->cfg.kernel_size), 256, 0, st, {},
+                    c->md.conv_k, c->md.conv_b, c->md.elt_w[ES_TRANSFORM], c->cfg.kernel_size,
+                    c->cfg.map_dim, c->Mp, c->conv_quad);
 }
 
 int check_ready(n2nmn_ctx* c) {
@@ -687,15 +695,18 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
   if (prop.major != 9)
     return fail(N2NMN_ERR_DEVICE, std::string("n2nmn_b200 needs an sm_90 GPU, found sm_") +
                                       std::to_string(prop.major) + std::to_string(prop.minor));
-  n2nmn_ctx* c = new n2nmn_ctx();
+  // every failure below frees what was built so far (n2nmn_destroy takes a partial context)
+  std::unique_ptr<n2nmn_ctx, int (*)(n2nmn_ctx*)> owner(new n2nmn_ctx(), n2nmn_destroy);
+  n2nmn_ctx* c = owner.get();
+  c->shp = sched_shape(*cfg);
   c->cfg = *cfg;
-  if (cfg->family == N2NMN_VQA) c->cfg.kernel_size = 1;
+  c->cfg.kernel_size = c->shp.ksize;
   c->device = cfg->device;
   c->num_sms = prop.multiProcessorCount;
   c->HW = cfg->H * cfg->W;
-  c->Dk = cfg->D + (cfg->family == N2NMN_VQA ? 2 : 0);
+  c->Dk = c->shp.Dk;
   c->Kp = round_up(c->Dk, kBK);
-  c->Mp = round_up(cfg->map_dim, 256);
+  c->Mp = c->shp.Mp;
   c->G = std::max(1, std::min(cfg->max_group, kMaxSeg));
   c->QB = c->G * cfg->max_batch;
   std::memset(&c->md, 0, sizeof(c->md));
@@ -703,8 +714,6 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
   md.H = cfg->H; md.W = cfg->W; md.HW = c->HW; md.Dk = c->Dk; md.Dt = cfg->text_dim;
   md.M = cfg->map_dim; md.Mp = c->Mp; md.C = cfg->num_choices; md.ksize = c->cfg.kernel_size;
   md.family = cfg->family;
-  c->shp = SchedShape{cfg->family, cfg->H, cfg->W, c->Dk, cfg->text_dim, cfg->map_dim, c->Mp,
-                      cfg->num_choices, c->cfg.kernel_size, cfg->max_T};
   build_variables(c);
   {   // flat TF-layout buffer (weights / gradients / Adam moments) and where each gradient goes
     int64_t off = 0;
@@ -761,8 +770,7 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
     CUDA_TRY(cudaMalloc(&c->proj_bias[s], (size_t)c->Mp * sizeof(float)));
     CUDA_TRY(cudaMemset(c->proj_bias[s], 0, (size_t)c->Mp * sizeof(float)));
     md.proj_b[s] = c->proj_bias[s];
-    if (int rc = encode_2d(c, &c->tmaps.b[s], c->proj_wt[s], c->Kp, c->Mp, c->Kp, kBK, kBNHalf))
-      return rc;
+    TRY(encode_2d(c, &c->tmaps.b[s], c->proj_wt[s], c->Kp, c->Mp, c->Kp, kBK, kBNHalf));
   }
   for (int s = 0; s < NUM_PROJ_SETS; ++s)      // sets the family lacks alias set 0 (never used)
     if (!c->proj_used[s]) c->tmaps.b[s] = c->tmaps.b[PS_FIND];
@@ -809,17 +817,14 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
           CUDA_TRY(cudaMemset(c->out_wt_hi[os], 0, wt));
           CUDA_TRY(cudaMemset(c->out_wt_lo[os], 0, wt));
           HeadTailMaps& hm = c->ht_maps[os];
-          if (int rc = encode_2d(c, &hm.a_hi, c->ehat, c->Mp, NB, c->Mp, kHtK, kHtM)) return rc;
-          if (int rc = encode_2d(c, &hm.a_lo, c->ehat_lo, c->Mp, NB, c->Mp, kHtK, kHtM)) return rc;
-          if (int rc = encode_2d(c, &hm.b_hi, c->out_wt_hi[os], c->Mp, c->Cpad, c->Mp, kHtK, kHtN)) return rc;
-          if (int rc = encode_2d(c, &hm.b_lo, c->out_wt_lo[os], c->Mp, c->Cpad, c->Mp, kHtK, kHtN)) return rc;
+          TRY(encode_2d(c, &hm.a_hi, c->ehat, c->Mp, NB, c->Mp, kHtK, kHtM));
+          TRY(encode_2d(c, &hm.a_lo, c->ehat_lo, c->Mp, NB, c->Mp, kHtK, kHtM));
+          TRY(encode_2d(c, &hm.b_hi, c->out_wt_hi[os], c->Mp, c->Cpad, c->Mp, kHtK, kHtN));
+          TRY(encode_2d(c, &hm.b_lo, c->out_wt_lo[os], c->Mp, c->Cpad, c->Mp, kHtK, kHtN));
         }
-    CUDA_TRY(cudaFuncSetAttribute(head_tail_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)kHtSmemBytes));
-    CUDA_TRY(cudaFuncSetAttribute(head_tail_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)mma_smem_bytes(2)));
-    CUDA_TRY(cudaFuncSetAttribute(head_tail_gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)mma_smem_bytes(4)));
+    TRY(set_smem(head_tail_wgmma_kernel, (int)kHtSmemBytes));
+    for (bool narrow : {true, false})
+      TRY(set_smem(tail_gemm_variant(narrow), (int)mma_smem_bytes(narrow ? 2 : 4)));
   }
   c->head_nn = head_nodes_per_cta(c->Dk, c->Mp);
   c->head_smem_bytes = head_smem_layout(c->head_nn, c->Kp, c->Mp).total * (int)sizeof(float);
@@ -852,50 +857,21 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
     if (c->tree_smem_bytes <= 200 * 1024 || c->stack_cap <= 2) break;
     --c->stack_cap;
   }
-  CUDA_TRY(cudaFuncSetAttribute(tree_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                c->tree_smem_bytes));
-  CUDA_TRY(cudaFuncSetAttribute(tree_kernel<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                c->tree_smem_bytes));
-  CUDA_TRY(cudaFuncSetAttribute(tree_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                c->tree_smem_bytes));
-  CUDA_TRY(cudaFuncSetAttribute(tree_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                c->tree_smem_bytes));
-  {
-    if (cfg->text_dim % 4 != 0)
-      return fail(N2NMN_ERR_ARG, "text_dim must be a multiple of 4 (16-byte word-vector rows)");
-    CUDA_TRY(cudaFuncSetAttribute(text_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)mma_smem_bytes(4, kTextStages)));
-    CUDA_TRY(cudaFuncSetAttribute(quad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)mma_smem_bytes(4, kTextStages)));
-    CUDA_TRY(cudaFuncSetAttribute(text_proj_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    CUDA_TRY(cudaFuncSetAttribute(quad_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+  for (int ks : {3, 5})
+    for (bool direct : {false, true}) TRY(set_smem(tree_variant(ks, direct), c->tree_smem_bytes));
+  if (cfg->text_dim % 4 != 0)
+    return fail(N2NMN_ERR_ARG, "text_dim must be a multiple of 4 (16-byte word-vector rows)");
+  TRY(set_smem(text_proj_kernel, (int)mma_smem_bytes(4, kTextStages), 100));
+  TRY(set_smem(quad_kernel, (int)mma_smem_bytes(4, kTextStages), 100));
+  for (int nn : {16, 8, 4}) {
+    const int bytes = head_smem_layout(nn, c->Kp, c->Mp).total * (int)sizeof(float);
+    TRY(set_smem(head_variant(nn), bytes <= 200 * 1024 ? bytes : 48 * 1024));
   }
-  CUDA_TRY(cudaFuncSetAttribute(head_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                head_smem_layout(16, c->Kp, c->Mp).total * (int)sizeof(float) <=
-                                        200 * 1024
-                                    ? head_smem_layout(16, c->Kp, c->Mp).total * (int)sizeof(float)
-                                    : 48 * 1024));
-  CUDA_TRY(cudaFuncSetAttribute(head_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                head_smem_layout(8, c->Kp, c->Mp).total * (int)sizeof(float) <=
-                                        200 * 1024
-                                    ? head_smem_layout(8, c->Kp, c->Mp).total * (int)sizeof(float)
-                                    : 48 * 1024));
-  CUDA_TRY(cudaFuncSetAttribute(head_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                head_smem_layout(4, c->Kp, c->Mp).total * (int)sizeof(float) <=
-                                        200 * 1024
-                                    ? head_smem_layout(4, c->Kp, c->Mp).total * (int)sizeof(float)
-                                    : 48 * 1024));
   if (c->head_smem_bytes > 200 * 1024)
     return fail(N2NMN_ERR_ARG, "feature depth too large for the answer-head kernel");
-  CUDA_TRY(cudaFuncSetAttribute(wave_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                c->node_smem_bytes));
-  CUDA_TRY(cudaFuncSetAttribute(wave_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                c->node_smem_bytes));
-  CUDA_TRY(cudaFuncSetAttribute(proj_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                proj_smem_bytes()));
-  CUDA_TRY(cudaFuncSetAttribute(
-      proj_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-      (int)((kSimtRows * kSimtKChunk + kSimtRows * c->Mp) * sizeof(float))));
+  for (int ks : {3, 5}) TRY(set_smem(wave_variant(ks), c->node_smem_bytes));
+  TRY(set_smem(proj_wgmma_kernel, proj_smem_bytes()));
+  TRY(set_smem(proj_simt_kernel, (int)((kSimtRows * kSimtKChunk + kSimtRows * c->Mp) * sizeof(float))));
   c->module_sched.uid = g_uid++;
   c->module_sched.shp = c->shp;
   c->step_sched.shp = c->shp;
@@ -907,7 +883,7 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
     const int v = std::atoi(e);
     if (v == 1 || v == 2 || v == 4 || v == 8) c->tree_cluster = v;
   }
-  *out = c;
+  *out = owner.release();
   return 0;
 }
 
@@ -927,7 +903,7 @@ int n2nmn_destroy(n2nmn_ctx* c) {
     cudaFree(c->out_wp[os]); cudaFree(c->out_wt_hi[os]); cudaFree(c->out_wt_lo[os]);
     cudaFree(c->out_wp_lo[os]);
   }
-  cudaFree(c->d_segs); cudaFree(c->d_sumsq);
+  cudaFree(c->d_segs); cudaFree(c->d_sumsq); cudaFree(c->d_repack);
   cudaFree(c->scores_tmp); cudaFree(c->e2e_feat); cudaFree(c->e2e_wv); cudaFree(c->e2e_scores);
   cudaFree(c->e2e_feat_f16);
   for (int i = 0; i < kTableSlots; ++i) {
@@ -962,37 +938,25 @@ int n2nmn_set_weight(n2nmn_ctx* c, const char* name, const float* src, const int
       if (shape[i] != v.shape[i]) return fail(N2NMN_ERR_ARG, std::string("shape mismatch for ") + name);
     if (v.kind == VK_PITCHED) {
       const int rows = (int)(v.count / (size_t)v.shape.back());
-      pitch_rows_kernel<<<(unsigned)rows, 256, 0, st>>>(src, rows, (int)v.shape.back(),
-                                                      c->wbuf + v.offset, c->Mp);
+      TRY(ctx_launch(c, pitch_rows_kernel, rows, 256, 0, st, {}, src, rows, (int)v.shape.back(),
+                     c->wbuf + v.offset, c->Mp));
     } else {
       CUDA_TRY(cudaMemcpyAsync(c->wbuf + v.offset, src, v.count * sizeof(float),
                                cudaMemcpyDeviceToDevice, st));
     }
     if (v.kind == VK_PROJ_W) {
-      dim3 grid((c->Kp + 31) / 32, (c->Mp + 31) / 32), block(32, 8);
-      transpose_pad_kernel<<<grid, block, 0, st>>>(c->wbuf + v.offset, c->Dk, c->cfg.map_dim,
-                                                   c->proj_wt[v.set], c->Kp, c->Mp);
+      TRY(ctx_launch(c, transpose_pad_kernel, dim3((c->Kp + 31) / 32, (c->Mp + 31) / 32), dim3(32, 8),
+                     0, st, {}, c->wbuf + v.offset, c->Dk, c->cfg.map_dim, c->proj_wt[v.set], c->Kp,
+                     c->Mp));
     } else if (v.kind == VK_PROJ_B) {
-      pad_copy_kernel<<<(c->Mp + 255) / 256, 256, 0, st>>>(c->wbuf + v.offset, c->cfg.map_dim,
-                                                           c->proj_bias[v.set], c->Mp);
+      TRY(ctx_launch(c, pad_copy_kernel, (c->Mp + 255) / 256, 256, 0, st, {}, c->wbuf + v.offset,
+                     c->cfg.map_dim, c->proj_bias[v.set], c->Mp));
     }
     for (int os = 0; os < NUM_OUT_SETS; ++os)
-      if (v.slot == &c->md.out_w[os] && c->out_wp[os]) {
-        pitch_rows_kernel<<<(unsigned)c->cfg.map_dim, 256, 0, st>>>(src, c->cfg.map_dim,
-                                                                   c->cfg.num_choices, c->out_wp[os], c->Cp);
-        if (c->out_wt_hi[os])
-          out_wt_split_kernel<<<dim3((c->Cpad + 31) / 32, (c->Mp + 31) / 32), dim3(32, 8), 0, st>>>(
-              src, c->cfg.map_dim, c->cfg.num_choices, c->out_wt_hi[os], c->out_wt_lo[os], c->Mp,
-              c->Cpad);
-      }
-    if (c->conv_quad && (v.slot == &c->md.conv_k || v.slot == &c->md.conv_b ||
-                         v.slot == &c->md.elt_w[ES_TRANSFORM])) {
-      // the Transform quadratic-form matrix depends on these three variables
-      conv_quad_kernel<<<quad_pitch(c->cfg.kernel_size), 256, 0, st>>>(
-          c->md.conv_k, c->md.conv_b, c->md.elt_w[ES_TRANSFORM], c->cfg.kernel_size,
-          c->cfg.map_dim, c->Mp, c->conv_quad);
-    }
-    CUDA_TRY(cudaGetLastError());
+      if (v.slot == &c->md.out_w[os]) TRY(pack_out_weights(c, os, src, st));
+    // the Transform quadratic-form matrix depends on these three variables
+    if (v.slot == &c->md.conv_k || v.slot == &c->md.conv_b || v.slot == &c->md.elt_w[ES_TRANSFORM])
+      TRY(update_conv_quad(c, st));
     v.loaded = true;
     return 0;
   }
@@ -1016,17 +980,15 @@ int bind_segments(n2nmn_ctx* c, int nseg, const float* const* feat, const float*
     const float* eff = feat[sgi];
     if (c->feat_aug) {
       float* dst = c->feat_aug + (size_t)sgi * c->cfg.max_batch * c->HW * c->Kp;
-      augment_features_kernel<<<rows, 128, 0, st>>>(feat[sgi], rows, c->cfg.D, c->cfg.H, c->cfg.W,
-                                                   c->cfg.family == N2NMN_VQA ? 1 : 0, dst, c->Kp);
-      CUDA_TRY(cudaGetLastError());
-      ++c->launches;
+      TRY(ctx_launch(c, augment_features_kernel, rows, 128, 0, st, {}, feat[sgi], rows, c->cfg.D,
+                     c->cfg.H, c->cfg.W, c->cfg.family == N2NMN_VQA ? 1 : 0, dst, c->Kp));
       eff = dst;
     }
     if ((reinterpret_cast<uintptr_t>(eff) & 15) != 0)
       return fail(N2NMN_ERR_ARG, "image_feat_grid must be 16-byte aligned");
     c->md.feat_seg[sgi] = eff;
     c->md.wv_seg[sgi] = wv[sgi];
-    if (int rc = encode_2d(c, &c->tmaps.a[sgi], eff, c->Dk, rows, pitch, kBK, kBM)) return rc;
+    TRY(encode_2d(c, &c->tmaps.a[sgi], eff, c->Dk, rows, pitch, kBK, kBM));
   }
   for (int sgi = nseg; sgi < kMaxSeg; ++sgi) {
     c->md.feat_seg[sgi] = c->md.feat_seg[0];
@@ -1071,10 +1033,7 @@ int n2nmn_compile_schedule_host(const n2nmn_config* cfg, const int32_t* tokens, 
                                 n2nmn_sched** out) {
   if (!cfg || !tokens || !vocab_ops || !out) return fail(N2NMN_ERR_ARG, "null argument");
   if (N <= 0 || T <= 0) return fail(N2NMN_ERR_ARG, "N and T must be positive");
-  const int Dk = cfg->D + (cfg->family == N2NMN_VQA ? 2 : 0);
-  const SchedShape shp{cfg->family, cfg->H, cfg->W, Dk, cfg->text_dim, cfg->map_dim,
-                       round_up(cfg->map_dim, 256), cfg->num_choices,
-                       cfg->family == N2NMN_VQA ? 1 : cfg->kernel_size, cfg->max_T};
+  const SchedShape shp = sched_shape(*cfg);
   n2nmn_sched* sc = new n2nmn_sched();
   sc->uid = g_uid++;
   sc->shp = shp;
@@ -1091,10 +1050,7 @@ int n2nmn_compile_schedule_host(const n2nmn_config* cfg, const int32_t* tokens, 
 double n2nmn_time_compile(const n2nmn_config* cfg, const int32_t* tokens, int T, int N,
                           const int32_t* vocab_ops, int num_vocab, int iters) {
   if (!cfg || !tokens || !vocab_ops || iters <= 0) return -1.0;
-  const int Dk = cfg->D + (cfg->family == N2NMN_VQA ? 2 : 0);
-  const SchedShape shp{cfg->family, cfg->H, cfg->W, Dk, cfg->text_dim, cfg->map_dim,
-                       round_up(cfg->map_dim, 256), cfg->num_choices,
-                       cfg->family == N2NMN_VQA ? 1 : cfg->kernel_size, cfg->max_T};
+  const SchedShape shp = sched_shape(*cfg);
   HostSchedule hs;
   const char* err = nullptr;
   compile_schedule(shp, tokens, T, N, vocab_ops, num_vocab, &hs, &err);
@@ -1112,8 +1068,6 @@ int n2nmn_compile_nodes(n2nmn_ctx* c, const int32_t* op, const int32_t* t_idx,
     return fail(N2NMN_ERR_ARG, "null argument");
   if (nq <= 0 || nq > c->cfg.max_batch) return fail(N2NMN_ERR_CAPACITY, "bad question count");
   if (q_ptr[0] != 0 || q_ptr[nq] != n) return fail(N2NMN_ERR_ARG, "q_ptr does not span the nodes");
-  static const int arity[NUM_OPS] = {0, 0, 1, 1, 1, 2, 2, 1, 1, 2, 2, 2, 2, 1};
-  static const bool is_ans[NUM_OPS] = {0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1};
   n2nmn_sched* sc = new n2nmn_sched();
   sc->uid = g_uid++;
   sc->shp = c->shp;
@@ -1134,18 +1088,18 @@ int n2nmn_compile_nodes(n2nmn_ctx* c, const int32_t* op, const int32_t* t_idx,
                 b_idx[i] >= 0 && b_idx[i] < c->cfg.max_batch;
       const int kids[2] = {in0[i], in1[i]};
       for (int k = 0; ok && k < 2; ++k) {
-        if (k < arity[o]) {
-          ok = kids[k] >= q_ptr[q] && kids[k] < i && !is_ans[op[kids[k]]];
+        if (k < kArity[o]) {
+          ok = kids[k] >= q_ptr[q] && kids[k] < i && !kIsAns[op[kids[k]]];
           if (ok) S.depth[i] = std::max(S.depth[i], S.depth[kids[k]] + 1);
         } else {
           ok = kids[k] < 0;
         }
       }
-      if (ok && is_ans[o] != (i == q_ptr[q + 1] - 1)) ok = false;   // exactly the root answers
+      if (ok && kIsAns[o] != (i == q_ptr[q + 1] - 1)) ok = false;   // exactly the root answers
       if (!ok) { delete sc; return fail(N2NMN_ERR_ARG, "malformed expression node " + std::to_string(i)); }
       r.op = o; r.t = t_idx[i]; r.b = b_idx[i];
       r.in0 = in0[i]; r.in1 = in1[i];
-      r.out = is_ans[o] ? q : i;
+      r.out = kIsAns[o] ? q : i;
       r.text = -1;
       r.aux = (o == OP_SCENE) ? scene_bits : -1;
       r.aux2 = -1; r.s0 = r.s1 = r.so = -1;
@@ -1242,10 +1196,8 @@ int module_fwd_impl(n2nmn_ctx* c, int op, const float* in0, const float* in1,
   if (n == 0) return 0;   // TF Fold's zero-size batches: nothing to do
   if (n < 0 || !out) return fail(N2NMN_ERR_ARG, "bad arguments");
   if (int rc = check_ready(c)) return rc;
-  static const int arity[NUM_OPS] = {0, 0, 1, 1, 1, 2, 2, 1, 1, 2, 2, 2, 2, 1};
-  static const bool is_ans[NUM_OPS] = {0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1};
   static const bool needs_idx[NUM_OPS] = {0, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0, 1, 1};
-  if ((arity[op] >= 1 && !in0) || (arity[op] >= 2 && !in1))
+  if ((kArity[op] >= 1 && !in0) || (kArity[op] >= 2 && !in1))
     return fail(N2NMN_ERR_ARG, "missing attention input");
   if (needs_idx[op] && (!t_idx || !b_idx))
     return fail(N2NMN_ERR_ARG, "time_idx / batch_idx required for this module");
@@ -1269,9 +1221,9 @@ int module_fwd_impl(n2nmn_ctx* c, int op, const float* in0, const float* in1,
     if (needs_idx[op] && (r.b < 0 || r.b >= c->N || r.t < 0 || r.t >= c->T))
       return fail(N2NMN_ERR_ARG, "time_idx / batch_idx out of range");
     if (!needs_idx[op]) { r.t = 0; r.b = 0; }
-    r.in0 = arity[op] >= 1 ? i : -1;
-    r.in1 = arity[op] >= 2 ? n + i : -1;
-    r.out = is_ans[op] ? i : 2 * n + i;
+    r.in0 = kArity[op] >= 1 ? i : -1;
+    r.in1 = kArity[op] >= 2 ? n + i : -1;
+    r.out = kIsAns[op] ? i : 2 * n + i;
     r.text = -1;
     r.aux = (op == OP_SCENE) ? scene_bits : -1;
     r.aux2 = -1; r.s0 = r.s1 = r.so = -1;
@@ -1280,14 +1232,14 @@ int module_fwd_impl(n2nmn_ctx* c, int op, const float* in0, const float* in1,
   S.q_ptr[n] = n;
   if (int rc = finalize_schedule(c->shp, c->N, &S)) return fail(rc, "finalize_schedule failed");
   const size_t map_bytes = (size_t)n * c->HW * sizeof(float);
-  if (arity[op] >= 1)
+  if (kArity[op] >= 1)
     CUDA_TRY(cudaMemcpyAsync(c->arena, in0, map_bytes, cudaMemcpyDeviceToDevice, st));
-  if (arity[op] >= 2)
+  if (kArity[op] >= 2)
     CUDA_TRY(cudaMemcpyAsync(c->arena + (size_t)n * c->HW, in1, map_bytes,
                              cudaMemcpyDeviceToDevice, st));
-  float* scores = is_ans[op] ? out : c->scores_tmp;
+  float* scores = kIsAns[op] ? out : c->scores_tmp;
   if (int rc = run_tables(c, sc, &scores, c->arena, st, /*force_wave=*/true)) return rc;
-  if (!is_ans[op])
+  if (!kIsAns[op])
     CUDA_TRY(cudaMemcpyAsync(out, c->arena + (size_t)2 * n * c->HW, map_bytes,
                              cudaMemcpyDeviceToDevice, st));
   return 0;
@@ -1349,16 +1301,13 @@ int forward_host_impl(n2nmn_ctx* c, int nb, const void* const* feat_host,
   const size_t fbytes = (size_t)N * c->HW * c->cfg.D * sizeof(float);
   const size_t wbytes = (size_t)T * N * c->cfg.text_dim * sizeof(float);
   const size_t sbytes = (size_t)N * c->cfg.num_choices * sizeof(float);
-  if (!c->e2e_feat) {
-    CUDA_TRY(cudaMalloc(&c->e2e_feat, c->G * fcap * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->e2e_wv, c->G * wcap * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->e2e_scores, c->G * scap * sizeof(float)));
-  }
+  CUDA_TRY(alloc_once(&c->e2e_feat, c->G * fcap * sizeof(float)));
+  CUDA_TRY(alloc_once(&c->e2e_wv, c->G * wcap * sizeof(float)));
+  CUDA_TRY(alloc_once(&c->e2e_scores, c->G * scap * sizeof(float)));
   if (feat_f16 && (fbytes / sizeof(float)) % 8 != 0)
     return fail(N2NMN_ERR_ARG, "fp16 host features need N*H*W*D to be a multiple of 8");
   const size_t fcap16 = (fcap + 7) & ~(size_t)7;   // fp16 staging slots stay 16-byte aligned
-  if (feat_f16 && !c->e2e_feat_f16)
-    CUDA_TRY(cudaMalloc(&c->e2e_feat_f16, c->G * fcap16 * sizeof(uint16_t)));
+  if (feat_f16) CUDA_TRY(alloc_once(&c->e2e_feat_f16, c->G * fcap16 * sizeof(uint16_t)));
   const float* fd[kMaxSeg];
   const float* wd[kMaxSeg];
   float* sd[kMaxSeg];
@@ -1376,12 +1325,10 @@ int forward_host_impl(n2nmn_ctx* c, int nb, const void* const* feat_host,
     const size_t cnt = fbytes / sizeof(float);
     for (int i = 0; i < nb; ++i) {
       const size_t n8 = (cnt + 7) / 8;
-      widen_f16_kernel<<<(unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)c->num_sms * 8), 256, 0, st>>>(
-          reinterpret_cast<const uint4*>(c->e2e_feat_f16 + i * fcap16),
-          reinterpret_cast<float4*>(c->e2e_feat + i * fcap), n8);
-      ++c->launches;
+      TRY(ctx_launch(c, widen_f16_kernel, (unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)c->num_sms * 8),
+                     256, 0, st, {}, reinterpret_cast<const uint4*>(c->e2e_feat_f16 + i * fcap16),
+                     reinterpret_cast<float4*>(c->e2e_feat + i * fcap), n8));
     }
-    CUDA_TRY(cudaGetLastError());
   }
   int rc = n2nmn_forward_group(c, nb, fd, wd, tokens, T, N, vocab_ops, num_vocab, sd, validity_out,
                                stream);
@@ -1449,7 +1396,7 @@ int n2nmn_flat_offset(const n2nmn_ctx* c, int index, int64_t* offset, int64_t* c
 namespace {
 int ensure_repack_tables(n2nmn_ctx* c) {
   const int nv = (int)c->vars.size();
-  if (!c->d_repack) {   // what n2nmn_set_weight does per variable, as device tables
+  if (!c->repack_ready) {   // what n2nmn_set_weight does per variable, as device tables
     std::vector<RepackSeg> segs(nv);
     ProjRepack& pr = c->proj_repack;
     for (int s = 0; s < NUM_PROJ_SETS; ++s) { pr.w_off[s] = pr.b_off[s] = -1; pr.wt[s] = pr.bias[s] = nullptr; }
@@ -1470,8 +1417,9 @@ int ensure_repack_tables(n2nmn_ctx* c) {
         pr.b_off[v.set] = (int)c->flat_offset[i];
       }
     }
-    CUDA_TRY(cudaMalloc(&c->d_repack, nv * sizeof(RepackSeg)));
+    CUDA_TRY(alloc_once(&c->d_repack, nv * sizeof(RepackSeg)));
     CUDA_TRY(cudaMemcpy(c->d_repack, segs.data(), nv * sizeof(RepackSeg), cudaMemcpyHostToDevice));
+    c->repack_ready = true;
   }
   return 0;
 }
@@ -1480,28 +1428,12 @@ int ensure_repack_tables(n2nmn_ctx* c) {
 int repack_derived(n2nmn_ctx* c, const float* wflat_dev, cudaStream_t st) {
   for (size_t i = 0; i < c->vars.size(); ++i)
     for (int os = 0; os < NUM_OUT_SETS; ++os)
-      if (c->vars[i].slot == &c->md.out_w[os] && c->out_wp[os]) {
-        pitch_rows_kernel<<<(unsigned)c->cfg.map_dim, 256, 0, st>>>(
-            wflat_dev + c->flat_offset[i], c->cfg.map_dim, c->cfg.num_choices, c->out_wp[os], c->Cp);
-        if (c->out_wt_hi[os])
-          out_wt_split_kernel<<<dim3((c->Cpad + 31) / 32, (c->Mp + 31) / 32), dim3(32, 8), 0, st>>>(
-              wflat_dev + c->flat_offset[i], c->cfg.map_dim, c->cfg.num_choices, c->out_wt_hi[os],
-              c->out_wt_lo[os], c->Mp, c->Cpad);
-        ++c->launches;
-      }
-  if (c->proj_repack_sets > 0) {
-    dim3 grid((c->Kp + 31) / 32, (c->Mp + 31) / 32, c->proj_repack_sets), block(32, 8);
-    proj_repack_kernel<<<grid, block, 0, st>>>(wflat_dev, c->proj_repack, c->Dk, c->cfg.map_dim,
-                                               c->Kp, c->Mp);
-    ++c->launches;
-  }
-  if (c->conv_quad) {
-    conv_quad_kernel<<<quad_pitch(c->cfg.kernel_size), 256, 0, st>>>(
-        c->md.conv_k, c->md.conv_b, c->md.elt_w[ES_TRANSFORM], c->cfg.kernel_size, c->cfg.map_dim,
-        c->Mp, c->conv_quad);
-    ++c->launches;
-  }
-  CUDA_TRY(cudaGetLastError());
+      if (c->vars[i].slot == &c->md.out_w[os]) TRY(pack_out_weights(c, os, wflat_dev + c->flat_offset[i], st));
+  if (c->proj_repack_sets > 0)
+    TRY(ctx_launch(c, proj_repack_kernel,
+                   dim3((c->Kp + 31) / 32, (c->Mp + 31) / 32, c->proj_repack_sets), dim3(32, 8), 0, st,
+                   {}, wflat_dev, c->proj_repack, c->Dk, c->cfg.map_dim, c->Kp, c->Mp));
+  TRY(update_conv_quad(c, st));
   for (Variable& v : c->vars) v.loaded = true;
   return 0;
 }
@@ -1510,10 +1442,9 @@ int repack_derived(n2nmn_ctx* c, const float* wflat_dev, cudaStream_t st) {
 int n2nmn_load_flat_weights(n2nmn_ctx* c, const float* wflat_dev, void* stream) {
   if (!c || !wflat_dev) return fail(N2NMN_ERR_ARG, "null argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = ensure_repack_tables(c)) return rc;
-  repack_all_kernel<<<dim3(16, (unsigned)c->vars.size()), 256, 0, st>>>(wflat_dev, c->d_repack,
-                                                                        c->wbuf, c->Mp);
-  ++c->launches;
+  TRY(ensure_repack_tables(c));
+  TRY(ctx_launch(c, repack_all_kernel, dim3(16, (unsigned)c->vars.size()), 256, 0, st, {}, wflat_dev,
+                 c->d_repack, c->wbuf, c->Mp));
   return repack_derived(c, wflat_dev, st);
 }
 
@@ -1526,6 +1457,203 @@ int n2nmn_train_backward(n2nmn_ctx* c, const float* feat_dev, const float* wv_de
                                  labels_host, invalid_expr_loss, scores_dev, gflat_dev, dword_dev,
                                  loss_dev, validity_out, nullptr, nullptr, stream);
 }
+
+namespace {
+// Training workspaces and kernel attributes, set up on the first backward pass.
+int ensure_train_workspace(n2nmn_ctx* c) {
+  if (c->train_ready) return 0;
+  const bool vqa = c->cfg.family == N2NMN_VQA;
+  const int NB = c->cfg.max_batch, C = c->cfg.num_choices;
+  CUDA_TRY(alloc_once(&c->dscores, (size_t)NB * C * sizeof(float)));
+  CUDA_TRY(alloc_once(&c->per_sample, (size_t)NB * sizeof(float)));
+  CUDA_TRY(alloc_once(&c->dtau, (size_t)c->text_rows_cap * c->Mp * sizeof(float)));
+  c->dmap_entries = NB * c->cfg.max_T;
+  CUDA_TRY(alloc_once(&c->dmap, (size_t)c->dmap_entries * c->HW * c->Mp * sizeof(float)));
+  if (!vqa)   // d(conv output) scratch of the conv Transform
+    CUDA_TRY(alloc_once(&c->dstencil, (size_t)c->dmap_entries * c->HW * c->Mp * sizeof(float)));
+  CUDA_TRY(alloc_once(&c->gmap, (size_t)c->arena_slots * ((c->HW + 3) & ~3) * sizeof(float)));
+  CUDA_TRY(alloc_once(&c->phi_buf, (size_t)NB * 2 * c->Mp * sizeof(float)));
+  c->wg_ok = c->Mp % kWgN == 0 && c->Dk >= kWgM;
+  if (c->wg_ok) TRY(set_smem(wgrad_wgmma_kernel, (int)kWgSmemBytes));
+  if (c->ehat) {   // many-class heads: the batched tail backward
+    const int zeros = std::max(c->Cp, c->Mp);
+    CUDA_TRY(alloc_once(&c->dehat, (size_t)NB * c->Mp * sizeof(float)));
+    CUDA_TRY(alloc_once(&c->ds_hi, (size_t)NB * c->Cp * sizeof(float)));
+    CUDA_TRY(alloc_once(&c->ds_lo, (size_t)NB * c->Cp * sizeof(float)));
+    CUDA_TRY(alloc_once(&c->tail_zero, (size_t)zeros * sizeof(float)));
+    CUDA_TRY(cudaMemset(c->tail_zero, 0, (size_t)zeros * sizeof(float)));
+    CUDA_TRY(alloc_once(&c->root_set, (size_t)NB * sizeof(int32_t)));
+    CUDA_TRY(alloc_once(&c->tail_dst, (size_t)NUM_OUT_SETS * NB * sizeof(float*)));
+    for (int os = 0; os < NUM_OUT_SETS; ++os) {
+      if (!c->out_wp[os]) continue;
+      const int M = c->cfg.map_dim;
+      CUDA_TRY(alloc_once(&c->out_wp_lo[os], (size_t)M * c->Cp * sizeof(float)));
+      HeadTailMaps& tm = c->tail_maps[os];
+      TRY(encode_2d(c, &tm.a_hi, c->ds_hi, c->Cp, NB, c->Cp, kHtK, kHtM));
+      TRY(encode_2d(c, &tm.a_lo, c->ds_lo, c->Cp, NB, c->Cp, kHtK, kHtM));
+      TRY(encode_2d(c, &tm.b_hi, c->out_wp[os], c->Cp, M, c->Cp, kHtK, kHtN));
+      TRY(encode_2d(c, &tm.b_lo, c->out_wp_lo[os], c->Cp, M, c->Cp, kHtK, kHtN));
+    }
+  }
+  const int ks = vqa ? 1 : c->cfg.kernel_size;
+  const int bwd_smem = (int)(bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, ks, C).total * sizeof(float));
+  if (vqa) {
+    for (bool wide : {false, true}) TRY(set_smem(bwd_variant(true, false, 1, wide), bwd_smem, 100));
+  } else {   // the Transform instantiations keep the default carveout
+    for (int k : {3, 5})
+      for (bool tr : {false, true}) TRY(set_smem(bwd_variant(false, tr, k, false), bwd_smem, tr ? -1 : 100));
+  }
+  TRY(set_smem(xtb_mma_kernel<FeatGradSrc>, (int)kXtbSmemBytes));
+  TRY(set_smem(xtb_mma_kernel<TextGradSrc>, (int)kXtbSmemBytes));
+  TRY(set_smem(xtb_mma_kernel<TailGradSrc>, (int)kXtbSmemBytes));
+  TRY(set_smem(text_xgrad_mma_kernel, (int)kXgSmemBytes));
+  c->train_ready = true;
+  return 0;
+}
+
+// Many-class heads: dê of every Describe-type root and the fc_eltwise gradients, batched.
+int bwd_answer_tail(n2nmn_ctx* c, const BwdCtx& bc, const DevTables& t, int N, float* gflat,
+                    cudaStream_t st) {
+  const int NB = c->cfg.max_batch, M = c->cfg.map_dim, C = c->cfg.num_choices;
+  TRY(ctx_launch(c, tail_prep_kernel, N, 256, 0, st, {}, bc, t.at<NodeRec>(t.o.nodes), t.at(t.o.q_ptr),
+                 c->Cp, NB, c->root_set, c->ehat, c->ds_hi, c->ds_lo, c->dehat, c->tail_dst));
+  prof_mark(c, "tail_prep_kernel", st);
+  TailGradSrc ts;
+  ts.md = c->md; ts.ehat = c->ehat; ts.ds = c->ds_hi; ts.root_set = c->root_set;
+  ts.zero_row = c->tail_zero; ts.nq = N; ts.Cp = c->Cp; ts.gflat = gflat; ts.go = c->go;
+  for (int os = 0; os < NUM_OUT_SETS; ++os) {
+    ts.has_set[os] = c->out_wp[os] != nullptr;
+    if (!c->out_wp[os]) continue;
+    const size_t n = (size_t)M * c->Cp;
+    TRY(ctx_launch(c, tf32_lo_kernel, (unsigned)std::min<size_t>((n + 255) / 256, 4 * (size_t)c->num_sms),
+                   256, 0, st, {}, c->out_wp[os], c->out_wp_lo[os], n));
+    // dÊ[q, :] = dS[q, :]·W_outᵀ for the questions whose root uses this set (3xTF32)
+    TRY(ctx_launch(c, head_tail_wgmma_kernel,
+                   dim3((unsigned)((M + kHtN - 1) / kHtN), (unsigned)((N + kHtM - 1) / kHtM)), kHtThreads,
+                   kHtSmemBytes, st, {}, c->tail_maps[os], c->tail_zero, c->tail_dst + (size_t)os * NB,
+                   0, N, M, C));
+  }
+  prof_mark(c, "tail_dehat_kernel", st);
+  // d(W_out) = Êᵀ·dS and d(b_out) = Σ_q dS, one segment per weight set
+  TRY(ctx_launch(c, xtb_mma_kernel<TailGradSrc>,
+                 dim3((M + kXtbM - 1) / kXtbM, (C + kXtbN - 1) / kXtbN, NUM_OUT_SETS), kXtbThreads,
+                 kXtbSmemBytes, st, {}, ts, 1));
+  prof_mark(c, "tail_wgrad_kernel", st);
+  return 0;
+}
+
+// The reverse tree walk, one launch per level, top down.
+int bwd_walk(n2nmn_ctx* c, const BwdCtx& bc, const HostSchedule& S, const DevTables& t,
+             cudaStream_t st) {
+  const bool vqa = c->cfg.family == N2NMN_VQA;
+  const BwdSmem L = bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, vqa ? 1 : c->cfg.kernel_size,
+                                    c->cfg.num_choices);
+  CUDA_TRY(cudaMemsetAsync(c->gmap, 0, S.nodes.size() * (size_t)L.HWp * sizeof(float), st));
+  CUDA_TRY(cudaMemsetAsync(c->dtau, 0, S.text_t.size() * (size_t)c->Mp * sizeof(float), st));
+  // a level's nodes are listed [Transform nodes | others]; a level with Transform nodes runs the
+  // full instantiation over all of them (one CTA per SM), a level without the lighter one
+  for (int dd = S.max_depth; dd >= 1; --dd) {
+    const int first = S.bwd_ptr[2 * dd], cnt = S.bwd_ptr[2 * dd + 2] - first;
+    if (cnt <= 0) continue;
+    const int n_tr = S.bwd_ptr[2 * dd + 1] - S.bwd_ptr[2 * dd];
+    // CTAs per splittable node: as many as keep the level's heavy CTAs within one wave of the
+    // SMs (one CTA per SM with Transform nodes, two without)
+    const int slices = n_tr > 0 ? std::max(3, std::min(kBwdSlicesMax, c->num_sms / n_tr))
+                                : std::max(2, std::min(6, 2 * c->num_sms / cnt));
+    TRY(ctx_launch(c, bwd_variant(vqa, n_tr > 0, c->cfg.kernel_size, c->Mp > 512), dim3(cnt, slices),
+                   kNodeThreads, L.total * sizeof(float), st, {c->use_pdl}, bc,
+                   t.at<NodeRec>(t.o.nodes), t.at(t.o.bwd_nodes), first, t.at(t.o.node_entry)));
+  }
+  prof_mark(c, "tree_bwd_kernel", st);
+  return 0;
+}
+
+// Text layers: weight gradients and, when asked for, d(word vectors).
+int bwd_text(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, float* gflat, float* dword,
+             cudaStream_t st) {
+  const int rows = (int)S.text_t.size();
+  if (rows == 0) return 0;
+  const int32_t *d_tt = t.at(t.o.text_t), *d_tb = t.at(t.o.text_b), *d_ss = t.at(t.o.text_set_start);
+  const int Dt = c->cfg.text_dim;
+  const bool exact = (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) != 0;
+  if (exact)
+    TRY(ctx_launch(c, text_wgrad_kernel, dim3((Dt + 7) / 8, NUM_TEXT_SETS), 256, 0, st, {}, c->md,
+                   c->dtau, d_tt, d_tb, d_ss, gflat, c->go));
+  else
+    TRY(ctx_launch(c, xtb_mma_kernel<TextGradSrc>,
+                   dim3((Dt + kXtbM - 1) / kXtbM, (c->cfg.map_dim + kXtbN - 1) / kXtbN, NUM_TEXT_SETS),
+                   kXtbThreads, kXtbSmemBytes, st, {},
+                   TextGradSrc{c->md, c->dtau, d_tt, d_tb, d_ss, gflat, c->go}, 1));
+  if (dword) {
+    if (exact) {
+      TRY(ctx_launch(c, text_xgrad_kernel, rows, 256, c->Mp * sizeof(float), st, {}, c->md, c->dtau,
+                     d_tt, d_tb, d_ss, dword, c->dword_scale));
+    } else {
+      TextSetRows tsr;
+      int groups = 0;
+      for (int i = 0; i <= NUM_TEXT_SETS; ++i) tsr.start[i] = S.text_set_start[i];
+      for (int i = 0; i < NUM_TEXT_SETS; ++i) groups += (tsr.start[i + 1] - tsr.start[i] + 63) / 64;
+      TRY(ctx_launch(c, text_xgrad_mma_kernel, dim3((Dt + 63) / 64, groups), kXgThreads, kXgSmemBytes,
+                     st, {}, c->md, c->dtau, d_tt, d_tb, tsr, dword, c->dword_scale));
+    }
+  }
+  prof_mark(c, "text_grad_kernels", st);
+  return 0;
+}
+
+// Feature-side layers: dW_set = Σ X^T·B, on CUDA cores (exact), wgmma or mma.sync.
+int bwd_features(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, float* gflat,
+                 cudaStream_t st) {
+  const int ne = (int)S.entries.size();
+  if (ne == 0) return 0;
+  const BwdEntry* d_ent = t.at<BwdEntry>(t.o.entries);
+  const int M = c->cfg.map_dim;
+  const bool exact = (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) != 0;
+  const bool wgmma = !exact && c->wg_ok && !std::getenv("N2NMN_WGRAD_MMA_SYNC");
+  if (exact) {
+    const int chunks = std::min(ne, 16);
+    const int per = (ne + chunks - 1) / chunks;
+    TRY(ctx_launch(c, feat_grad_kernel,
+                   dim3((c->Dk + kFgTile - 1) / kFgTile, (M + kFgTile - 1) / kFgTile, (ne + per - 1) / per),
+                   256, 0, st, {}, c->md, c->dmap, d_ent, ne, per, gflat, c->go));
+  } else if (wgmma) {
+    // both operands staged transposed (K-major) from the feature grid and the B maps
+    const int slabs = (c->Dk + kWgM - 1) / kWgM, ntiles = c->Mp / kWgN, tiles = slabs * ntiles;
+    int chunks = std::max(1, std::min(ne, c->num_sms / tiles));
+    if (chunks < 4) {   // few entry chunks per tile: pick the count that wastes the least of the waves
+      double best = 1e30;
+      for (int k = 1; k <= std::min(ne, 8); ++k) {
+        const double cost = (double)((tiles * k + c->num_sms - 1) / c->num_sms) / k;
+        if (cost < best - 1e-9) { best = cost; chunks = k; }
+      }
+    }
+    WgradParams wp;
+    wp.feat = c->md.feat; wp.dmap = c->dmap; wp.entries = d_ent;
+    wp.order = t.at(t.o.entry_order);
+    wp.num_entries = ne; wp.per_cta = (ne + chunks - 1) / chunks;
+    wp.HW = c->HW; wp.Dk = c->Dk; wp.M = M; wp.Mp = c->Mp;
+    wp.pitch = c->md.feat_pitch; wp.gflat = gflat; wp.go = c->go;
+    TRY(ctx_launch(c, wgrad_wgmma_kernel, dim3(slabs, (ne + wp.per_cta - 1) / wp.per_cta, ntiles),
+                   kWgThreads, kWgSmemBytes, st, {}, wp));
+  } else {
+    // two CTAs per SM (106 KB of ring each): ~2 x SMs CTAs over (Dk/128) x (M/64) tiles
+    const int tiles = ((c->Dk + kXtbM - 1) / kXtbM) * ((M + kXtbN - 1) / kXtbN);
+    const int chunks = std::max(1, std::min(ne, (2 * c->num_sms + tiles - 1) / tiles));
+    const int per = (ne + chunks - 1) / chunks;
+    TRY(ctx_launch(c, xtb_mma_kernel<FeatGradSrc>,
+                   dim3((c->Dk + kXtbM - 1) / kXtbM, (M + kXtbN - 1) / kXtbN, (ne + per - 1) / per),
+                   kXtbThreads, kXtbSmemBytes, st, {},
+                   FeatGradSrc{c->md, c->dmap, d_ent, ne, gflat, c->go}, per));
+  }
+  prof_mark(c, "feat_grad_kernel", st);
+  if (wgmma) {   // the wgmma kernel leaves the bias gradients to a column sum of the B maps
+    TRY(ctx_launch(c, bmap_colsum_kernel, ne, 1024, 0, st, {}, c->dmap, d_ent, c->HW, M, c->Mp, gflat,
+                   c->go));
+    prof_mark(c, "bias_grad_kernel", st);
+  }
+  return 0;
+}
+}  // namespace
 
 int n2nmn_train_backward_ex(n2nmn_ctx* c, const float* feat_dev, const float* wv_dev,
                             const int32_t* tokens, int T, int N, const int32_t* vocab_ops,
@@ -1544,92 +1672,16 @@ int n2nmn_train_backward_ex(n2nmn_ctx* c, const float* feat_dev, const float* wv
     return fail(N2NMN_ERR_ARG,
                 "n2nmn_train_backward: map_dim > 512 is not supported for the conv-Transform families");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = n2nmn_bind_inputs(c, feat_dev, wv_dev, N, T, stream)) return rc;
-  if (int rc = check_ready(c)) return rc;
-  const int NB = c->cfg.max_batch, TT = c->cfg.max_T, C = c->cfg.num_choices;
-  const int KSb = vqa ? 1 : c->cfg.kernel_size;
-  const bool wide = c->Mp > 512;
-  if (!c->dscores) {
-    CUDA_TRY(cudaMalloc(&c->dscores, (size_t)NB * C * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->per_sample, (size_t)NB * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->dtau, (size_t)c->text_rows_cap * c->Mp * sizeof(float)));
-    c->dmap_entries = NB * TT;
-    CUDA_TRY(cudaMalloc(&c->dmap, (size_t)c->dmap_entries * c->HW * c->Mp * sizeof(float)));
-    if (!vqa)   // d(conv output) scratch of the conv Transform
-      CUDA_TRY(cudaMalloc(&c->dstencil, (size_t)c->dmap_entries * c->HW * c->Mp * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->gmap, (size_t)c->arena_slots * ((c->HW + 3) & ~3) * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->phi_buf, (size_t)NB * 2 * c->Mp * sizeof(float)));
-    c->wg_ok = c->Mp % kWgN == 0 && c->Dk >= kWgM;
-    if (c->wg_ok)
-      CUDA_TRY(cudaFuncSetAttribute(wgrad_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)kWgSmemBytes));
-    if (c->ehat) {   // many-class heads: the batched tail backward
-      const int zeros = std::max(c->Cp, c->Mp);
-      CUDA_TRY(cudaMalloc(&c->dehat, (size_t)NB * c->Mp * sizeof(float)));
-      CUDA_TRY(cudaMalloc(&c->ds_hi, (size_t)NB * c->Cp * sizeof(float)));
-      CUDA_TRY(cudaMalloc(&c->ds_lo, (size_t)NB * c->Cp * sizeof(float)));
-      CUDA_TRY(cudaMalloc(&c->tail_zero, (size_t)zeros * sizeof(float)));
-      CUDA_TRY(cudaMemset(c->tail_zero, 0, (size_t)zeros * sizeof(float)));
-      CUDA_TRY(cudaMalloc(&c->root_set, (size_t)NB * sizeof(int32_t)));
-      CUDA_TRY(cudaMalloc(&c->tail_dst, (size_t)NUM_OUT_SETS * NB * sizeof(float*)));
-      for (int os = 0; os < NUM_OUT_SETS; ++os) {
-        if (!c->out_wp[os]) continue;
-        const size_t n = (size_t)c->cfg.map_dim * c->Cp;
-        CUDA_TRY(cudaMalloc(&c->out_wp_lo[os], n * sizeof(float)));
-        HeadTailMaps& tm = c->tail_maps[os];
-        const int M = c->cfg.map_dim;
-        if (int rc = encode_2d(c, &tm.a_hi, c->ds_hi, c->Cp, NB, c->Cp, kHtK, kHtM)) return rc;
-        if (int rc = encode_2d(c, &tm.a_lo, c->ds_lo, c->Cp, NB, c->Cp, kHtK, kHtM)) return rc;
-        if (int rc = encode_2d(c, &tm.b_hi, c->out_wp[os], c->Cp, M, c->Cp, kHtK, kHtN)) return rc;
-        if (int rc = encode_2d(c, &tm.b_lo, c->out_wp_lo[os], c->Cp, M, c->Cp, kHtK, kHtN)) return rc;
-      }
-    }
-    const BwdSmem L = bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, KSb, C);
-    const int bwd_smem = (int)(L.total * sizeof(float));
-    if (vqa) {
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<1, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<1, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    } else {
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem));
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<3, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-      CUDA_TRY(cudaFuncSetAttribute(tree_bwd_kernel<5, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    }
-    CUDA_TRY(cudaFuncSetAttribute(xtb_mma_kernel<FeatGradSrc>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kXtbSmemBytes));
-    CUDA_TRY(cudaFuncSetAttribute(xtb_mma_kernel<TextGradSrc>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kXtbSmemBytes));
-    CUDA_TRY(cudaFuncSetAttribute(xtb_mma_kernel<TailGradSrc>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kXtbSmemBytes));
-    CUDA_TRY(cudaFuncSetAttribute(text_xgrad_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)kXgSmemBytes));
-  }
+  TRY(n2nmn_bind_inputs(c, feat_dev, wv_dev, N, T, stream));
+  TRY(check_ready(c));
+  const int C = c->cfg.num_choices;
+  TRY(ensure_train_workspace(c));
   n2nmn_sched* sc = &c->step_sched;
   sc->uid = g_uid++;
   const char* err = nullptr;
   if (int rc = compile_schedule(c->shp, tokens, T, N, vocab_ops, num_vocab, &sc->hs, &err, true))
     return fail(rc, err ? err : "compile_schedule failed");
-  {   // every node bucketed by depth (leaves = 1): the backward runs one launch per level, top down
-    HostSchedule& W = sc->hs;
-    // bucket 2*depth: the level's Transform nodes (the long CTAs: scheduled first), 2*depth + 1:
-    // its other nodes
-    const int nb = 2 * (W.max_depth + 1);
-    W.bwd_ptr.assign(nb + 1, 0);
-    auto bucket = [&](size_t i) { return 2 * W.depth[i] + (W.nodes[i].op == OP_TRANSFORM ? 0 : 1); };
-    for (size_t i = 0; i < W.nodes.size(); ++i) ++W.bwd_ptr[bucket(i) + 1];
-    for (int b = 0; b < nb; ++b) W.bwd_ptr[b + 1] += W.bwd_ptr[b];
-    W.bwd_nodes.assign(W.nodes.size(), 0);
-    std::vector<int32_t> fill(W.bwd_ptr.begin(), W.bwd_ptr.end() - 1);
-    for (size_t i = 0; i < W.nodes.size(); ++i) W.bwd_nodes[fill[bucket(i)]++] = (int32_t)i;
-    W.entry_order.resize(W.entries.size());
-    for (size_t i = 0; i < W.entries.size(); ++i) W.entry_order[i] = (int32_t)i;
-    std::stable_sort(W.entry_order.begin(), W.entry_order.end(),
-                     [&](int32_t a, int32_t b) { return W.entries[a].set < W.entries[b].set; });
-  }
+  build_bwd_order(&sc->hs);
   const HostSchedule& S = sc->hs;
   if (validity_out) std::memcpy(validity_out, S.validity.data(), N);
   if ((int)S.nodes.size() > c->arena_slots || (int)S.entries.size() > c->dmap_entries ||
@@ -1644,10 +1696,7 @@ int n2nmn_train_backward_ex(n2nmn_ctx* c, const float* feat_dev, const float* wv
   const int rc = run_tables(c, sc, &scores_dev, c->arena, st, false, /*write_arena=*/true);
   c->train_labels = nullptr;
   if (rc) return rc;
-  const uint8_t* d = c->last_tables;
-  const TableOffsets& o = c->last_offsets;
-  const NodeRec* d_nodes = reinterpret_cast<const NodeRec*>(d + o.nodes);
-  const int32_t* d_qptr = reinterpret_cast<const int32_t*>(d + o.q_ptr);
+  const DevTables t{c->last_tables, c->last_offsets};
   // ---- loss and d(scores)
   CUDA_TRY(cudaMemsetAsync(gflat_dev, 0, (size_t)c->flat_size * sizeof(float), st));
   CUDA_TRY(cudaMemsetAsync(loss_dev, 0, sizeof(float), st));
@@ -1655,177 +1704,23 @@ int n2nmn_train_backward_ex(n2nmn_ctx* c, const float* feat_dev, const float* wv
     CUDA_TRY(cudaMemsetAsync(dword_dev, 0, (size_t)T * N * c->cfg.text_dim * sizeof(float), st));
   // VQA: cross-entropy on every row (exp_vqa/train_vqa_rl_gt_layout.py:101-116; invalid_expr_loss
   // only seeds the baseline there)
-  loss_kernel<<<(N + 7) / 8, 256, 0, st>>>(scores_dev, score_prior_dev,
-                                           reinterpret_cast<const int32_t*>(d + o.labels), d_qptr, N,
-                                           C, invalid_expr_loss, vqa ? 1 : 0, c->dscores, dscores_dev,
-                                           c->dword_scale, loss_dev + 1, loss_dev);
-  ++c->launches;
+  TRY(ctx_launch(c, loss_kernel, (N + 7) / 8, 256, 0, st, {}, scores_dev, score_prior_dev,
+                 t.at(t.o.labels), t.at(t.o.q_ptr), N, C, invalid_expr_loss, vqa ? 1 : 0, c->dscores,
+                 dscores_dev, c->dword_scale, loss_dev + 1, loss_dev));
   prof_mark(c, "loss_kernel", st);
   BwdCtx bc;
   bc.md = c->md; bc.tb = c->tb; bc.arena = c->arena; bc.scores = scores_dev;
   bc.dscores = c->dscores; bc.mbuf = c->mbuf; bc.gflat = gflat_dev; bc.dtau = c->dtau;
   bc.dmap = c->dmap; bc.dstencil = c->dstencil; bc.gmap = c->gmap; bc.phi = c->phi_buf; bc.go = c->go;
   bc.dehat = nullptr;
-  // ---- many-class heads: dê of every Describe-type root and the fc_eltwise gradients, batched
-  // (the exact-fp32 verification path keeps the per-root CUDA-core loop of the walk)
+  // the exact-fp32 verification path keeps the per-root CUDA-core loop of the walk
   if (c->ehat && !(c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT)) {
-    tail_prep_kernel<<<N, 256, 0, st>>>(bc, d_nodes, d_qptr, c->Cp, NB, c->root_set, c->ehat,
-                                        c->ds_hi, c->ds_lo, c->dehat, c->tail_dst);
-    ++c->launches;
-    prof_mark(c, "tail_prep_kernel", st);
-    TailGradSrc ts;
-    ts.md = c->md; ts.ehat = c->ehat; ts.ds = c->ds_hi; ts.root_set = c->root_set;
-    ts.zero_row = c->tail_zero; ts.nq = N; ts.Cp = c->Cp; ts.gflat = gflat_dev; ts.go = c->go;
-    for (int os = 0; os < NUM_OUT_SETS; ++os) {
-      ts.has_set[os] = c->out_wp[os] != nullptr;
-      if (!c->out_wp[os]) continue;
-      const size_t n = (size_t)c->cfg.map_dim * c->Cp;
-      tf32_lo_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, 4 * (size_t)c->num_sms), 256, 0, st>>>(
-          c->out_wp[os], c->out_wp_lo[os], n);
-      // dÊ[q, :] = dS[q, :]·W_outᵀ for the questions whose root uses this set (3xTF32)
-      head_tail_wgmma_kernel<<<dim3((unsigned)((c->cfg.map_dim + kHtN - 1) / kHtN),
-                                    (unsigned)((N + kHtM - 1) / kHtM)),
-                               kHtThreads, kHtSmemBytes, st>>>(
-          c->tail_maps[os], c->tail_zero, c->tail_dst + (size_t)os * NB, 0, N, c->cfg.map_dim, C);
-      c->launches += 2;
-    }
-    prof_mark(c, "tail_dehat_kernel", st);
-    // d(W_out) = Êᵀ·dS and d(b_out) = Σ_q dS, one segment per weight set
-    dim3 gt((c->cfg.map_dim + kXtbM - 1) / kXtbM, (C + kXtbN - 1) / kXtbN, NUM_OUT_SETS);
-    xtb_mma_kernel<TailGradSrc><<<gt, kXtbThreads, kXtbSmemBytes, st>>>(ts, 1);
-    ++c->launches;
-    CUDA_TRY(cudaGetLastError());
-    prof_mark(c, "tail_wgrad_kernel", st);
+    TRY(bwd_answer_tail(c, bc, t, N, gflat_dev, st));
     bc.dehat = c->dehat;
   }
-  // ---- reverse tree walk
-  const BwdSmem L = bwd_smem_layout(c->cfg.H, c->cfg.W, c->Mp, KSb, C);
-  const size_t bsm = L.total * sizeof(float);
-  const int32_t* d_entry = reinterpret_cast<const int32_t*>(d + o.node_entry);
-  const int32_t* d_bwd = reinterpret_cast<const int32_t*>(d + o.bwd_nodes);
-  CUDA_TRY(cudaMemsetAsync(c->gmap, 0, S.nodes.size() * (size_t)L.HWp * sizeof(float), st));
-  CUDA_TRY(cudaMemsetAsync(c->dtau, 0, S.text_t.size() * (size_t)c->Mp * sizeof(float), st));
-  // a level's nodes are listed [Transform nodes | others]; a level with Transform nodes runs the
-  // full instantiation over all of them (one CTA per SM), a level without the lighter one
-  for (int dd = S.max_depth; dd >= 1; --dd) {
-    const int first = S.bwd_ptr[2 * dd], cnt = S.bwd_ptr[2 * dd + 2] - first;
-    if (cnt <= 0) continue;
-    const int n_tr = S.bwd_ptr[2 * dd + 1] - S.bwd_ptr[2 * dd];
-    const bool has_tr = n_tr > 0;
-    // CTAs per splittable node: as many as keep the level's heavy CTAs within one wave of the
-    // SMs (one CTA per SM with Transform nodes, two without)
-    const int slices = has_tr ? std::max(3, std::min(kBwdSlicesMax, c->num_sms / n_tr))
-                              : std::max(2, std::min(6, 2 * c->num_sms / cnt));
-    cudaLaunchConfig_t bl;
-    std::memset(&bl, 0, sizeof(bl));
-    bl.gridDim = dim3(cnt, slices);
-    bl.blockDim = dim3(kNodeThreads);
-    bl.dynamicSmemBytes = bsm;
-    bl.stream = st;
-    cudaLaunchAttribute battr[1];
-    battr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    battr[0].val.programmaticStreamSerializationAllowed = 1;
-    bl.attrs = battr;
-    bl.numAttrs = c->use_pdl ? 1 : 0;
-    const bool k5 = c->cfg.kernel_size == 5;
-    if (vqa) {
-      if (wide) CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<1, false, true>, bc, d_nodes, d_bwd, first, d_entry));
-      else CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<1, false, false>, bc, d_nodes, d_bwd, first, d_entry));
-    } else if (has_tr) {
-      if (k5) CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<5, true>, bc, d_nodes, d_bwd, first, d_entry));
-      else CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<3, true>, bc, d_nodes, d_bwd, first, d_entry));
-    } else {
-      if (k5) CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<5, false>, bc, d_nodes, d_bwd, first, d_entry));
-      else CUDA_TRY(cudaLaunchKernelEx(&bl, tree_bwd_kernel<3, false>, bc, d_nodes, d_bwd, first, d_entry));
-    }
-    ++c->launches;
-  }
-  prof_mark(c, "tree_bwd_kernel", st);
-  // ---- text layers
-  const int rows = (int)S.text_t.size();
-  if (rows > 0) {
-    const int32_t* d_tt = reinterpret_cast<const int32_t*>(d + o.text_t);
-    const int32_t* d_tb = reinterpret_cast<const int32_t*>(d + o.text_b);
-    const int32_t* d_ss = reinterpret_cast<const int32_t*>(d + o.text_set_start);
-    const bool exact = (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) != 0;
-    if (exact) {
-      dim3 g1((c->cfg.text_dim + 7) / 8, NUM_TEXT_SETS);
-      text_wgrad_kernel<<<g1, 256, 0, st>>>(c->md, c->dtau, d_tt, d_tb, d_ss, gflat_dev, c->go);
-    } else {
-      TextGradSrc ts{c->md, c->dtau, d_tt, d_tb, d_ss, gflat_dev, c->go};
-      dim3 g1((c->cfg.text_dim + kXtbM - 1) / kXtbM, (c->cfg.map_dim + kXtbN - 1) / kXtbN,
-              NUM_TEXT_SETS);
-      xtb_mma_kernel<TextGradSrc><<<g1, kXtbThreads, kXtbSmemBytes, st>>>(ts, 1);
-    }
-    ++c->launches;
-    if (dword_dev) {
-      if (exact) {
-        text_xgrad_kernel<<<rows, 256, c->Mp * sizeof(float), st>>>(c->md, c->dtau, d_tt, d_tb, d_ss,
-                                                                   dword_dev, c->dword_scale);
-      } else {
-        TextSetRows tsr;
-        int groups = 0;
-        for (int i = 0; i <= NUM_TEXT_SETS; ++i) tsr.start[i] = S.text_set_start[i];
-        for (int i = 0; i < NUM_TEXT_SETS; ++i) groups += (tsr.start[i + 1] - tsr.start[i] + 63) / 64;
-        dim3 g3((c->cfg.text_dim + 63) / 64, groups);
-        text_xgrad_mma_kernel<<<g3, kXgThreads, kXgSmemBytes, st>>>(c->md, c->dtau, d_tt, d_tb, tsr,
-                                                                    dword_dev, c->dword_scale);
-      }
-      ++c->launches;
-    }
-    prof_mark(c, "text_grad_kernels", st);
-  }
-  // ---- feature-side layers: dW_set = Σ X^T·B
-  const int ne = (int)S.entries.size();
-  if (ne > 0) {
-    const BwdEntry* d_ent = reinterpret_cast<const BwdEntry*>(d + o.entries);
-    if (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) {
-      const int chunks = std::min(ne, 16);
-      const int per = (ne + chunks - 1) / chunks;
-      dim3 g2((c->Dk + kFgTile - 1) / kFgTile, (c->cfg.map_dim + kFgTile - 1) / kFgTile,
-              (ne + per - 1) / per);
-      feat_grad_kernel<<<g2, 256, 0, st>>>(c->md, c->dmap, d_ent, ne, per, gflat_dev, c->go);
-    } else if (c->wg_ok && !std::getenv("N2NMN_WGRAD_MMA_SYNC")) {
-      // wgmma, both operands staged transposed (K-major) from the feature grid and the B maps
-      const int slabs = (c->Dk + kWgM - 1) / kWgM, ntiles = c->Mp / kWgN, tiles = slabs * ntiles;
-      int chunks = std::max(1, std::min(ne, c->num_sms / tiles));
-      if (chunks < 4) {   // few entry chunks per tile: pick the count that wastes the least of the waves
-        double best = 1e30;
-        for (int k = 1; k <= std::min(ne, 8); ++k) {
-          const double cost = (double)((tiles * k + c->num_sms - 1) / c->num_sms) / k;
-          if (cost < best - 1e-9) { best = cost; chunks = k; }
-        }
-      }
-      WgradParams wp;
-      wp.feat = c->md.feat; wp.dmap = c->dmap; wp.entries = d_ent;
-      wp.order = reinterpret_cast<const int32_t*>(d + o.entry_order);
-      wp.num_entries = ne; wp.per_cta = (ne + chunks - 1) / chunks;
-      wp.HW = c->HW; wp.Dk = c->Dk; wp.M = c->cfg.map_dim; wp.Mp = c->Mp;
-      wp.pitch = c->md.feat_pitch; wp.gflat = gflat_dev; wp.go = c->go;
-      dim3 gw(slabs, (ne + wp.per_cta - 1) / wp.per_cta, ntiles);
-      wgrad_wgmma_kernel<<<gw, kWgThreads, kWgSmemBytes, st>>>(wp);
-      prof_mark(c, "feat_grad_kernel", st);
-      bmap_colsum_kernel<<<ne, 1024, 0, st>>>(c->dmap, d_ent, c->HW, c->cfg.map_dim, c->Mp, gflat_dev,
-                                             c->go);
-      c->launches += 2;
-      prof_mark(c, "bias_grad_kernel", st);
-      CUDA_TRY(cudaGetLastError());
-      return 0;
-    } else {
-      // two CTAs per SM (106 KB of ring each): ~2 x SMs CTAs over (Dk/128) x (M/64) tiles
-      const int tiles = ((c->Dk + kXtbM - 1) / kXtbM) * ((c->cfg.map_dim + kXtbN - 1) / kXtbN);
-      const int chunks = std::max(1, std::min(ne, (2 * c->num_sms + tiles - 1) / tiles));
-      const int per = (ne + chunks - 1) / chunks;
-      FeatGradSrc fs{c->md, c->dmap, d_ent, ne, gflat_dev, c->go};
-      dim3 g2((c->Dk + kXtbM - 1) / kXtbM, (c->cfg.map_dim + kXtbN - 1) / kXtbN,
-              (ne + per - 1) / per);
-      xtb_mma_kernel<FeatGradSrc><<<g2, kXtbThreads, kXtbSmemBytes, st>>>(fs, per);
-    }
-    ++c->launches;
-    prof_mark(c, "feat_grad_kernel", st);
-  }
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+  TRY(bwd_walk(c, bc, S, t, st));
+  TRY(bwd_text(c, S, t, gflat_dev, dword_dev, st));
+  return bwd_features(c, S, t, gflat_dev, st);
 }
 
 namespace {
@@ -1833,7 +1728,7 @@ int adam_impl(n2nmn_ctx* c, float* wflat, float* gflat, float* m, float* v, int 
               float beta1, float beta2, float eps, float max_norm, float weight_decay, float gscale,
               float* l2_dev, cudaStream_t st) {
   const int nv = (int)c->vars.size();
-  if (!c->d_segs) {
+  if (!c->segs_ready) {
     std::vector<VarSeg> segs(nv);
     for (int i = 0; i < nv; ++i) {
       segs[i].offset = (int)c->flat_offset[i];
@@ -1841,21 +1736,21 @@ int adam_impl(n2nmn_ctx* c, float* wflat, float* gflat, float* m, float* v, int 
       const std::string& n = c->vars[i].name;   // l2_reg covers ".../weights" only
       segs[i].decay = n.size() >= 8 && n.compare(n.size() - 8, 8, "/weights") == 0;
     }
-    CUDA_TRY(cudaMalloc(&c->d_segs, nv * sizeof(VarSeg)));
+    CUDA_TRY(alloc_once(&c->d_segs, nv * sizeof(VarSeg)));
     CUDA_TRY(cudaMemcpy(c->d_segs, segs.data(), nv * sizeof(VarSeg), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMalloc(&c->d_sumsq, nv * sizeof(float)));
+    CUDA_TRY(alloc_once(&c->d_sumsq, nv * sizeof(float)));
+    c->segs_ready = true;
   }
   CUDA_TRY(cudaMemsetAsync(c->d_sumsq, 0, nv * sizeof(float), st));
-  dim3 grid(32, nv);
-  grad_norm_kernel<<<grid, 256, 0, st>>>(wflat, gflat, c->d_segs, weight_decay, gscale, c->d_sumsq,
-                                         l2_dev);
+  const dim3 grid(32, nv);
+  TRY(ctx_launch(c, grad_norm_kernel, grid, 256, 0, st, {}, wflat, gflat, c->d_segs,
+                 weight_decay, gscale, c->d_sumsq, l2_dev));
   const double lr_t = (double)lr * std::sqrt(1.0 - std::pow((double)beta2, step)) /
                       (1.0 - std::pow((double)beta1, step));
-  if (int rc = ensure_repack_tables(c)) return rc;
-  adam_clip_kernel<<<grid, 256, 0, st>>>(wflat, gflat, m, v, c->d_segs, c->d_sumsq, (float)lr_t,
-                                         beta1, beta2, eps, max_norm, c->d_repack, c->wbuf, c->Mp);
-  c->launches += 2;
-  CUDA_TRY(cudaGetLastError());
+  TRY(ensure_repack_tables(c));
+  TRY(ctx_launch(c, adam_clip_kernel, grid, 256, 0, st, {}, wflat, gflat, m, v,
+                 c->d_segs, c->d_sumsq, (float)lr_t, beta1, beta2, eps, max_norm,
+                 c->d_repack, c->wbuf, c->Mp));
   prof_mark(c, "clip_adam_kernels", st);
   const int rc = repack_derived(c, wflat, st);
   prof_mark(c, "repack_kernels", st);
@@ -1881,9 +1776,8 @@ int n2nmn_train_finish(n2nmn_ctx* c, float* wflat, float* gflat, float* m, float
       !state_in_dev || !state_out_dev || N <= 0 || world <= 0)
     return fail(N2NMN_ERR_ARG, "bad argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  train_scalars_kernel<<<1, 256, 0, st>>>(loss_sum_dev, per_sample_dev, log_seq_prob_dev, N, world,
-                                          baseline_decay, state_in_dev, state_out_dev, coeff_dev);
-  ++c->launches;
+  TRY(ctx_launch(c, train_scalars_kernel, 1, 256, 0, st, {}, loss_sum_dev, per_sample_dev,
+                 log_seq_prob_dev, N, world, baseline_decay, state_in_dev, state_out_dev, coeff_dev));
   return adam_impl(c, wflat, gflat, m, v, step, lr, beta1, beta2, eps, max_norm, weight_decay,
                    1.f / (float)world, state_out_dev + 3, st);
 }
@@ -1947,3 +1841,4 @@ int n2nmn_get_launch_times(n2nmn_ctx* c, const char** names, float* us, int cap)
 int64_t n2nmn_launch_count(const n2nmn_ctx* c) { return c ? c->launches : 0; }
 
 }  // extern "C"
+

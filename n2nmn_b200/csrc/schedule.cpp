@@ -8,10 +8,6 @@ namespace n2nmn {
 
 namespace {
 
-const int kArity[NUM_OPS] = {0, 0, 1, 1, 1, 2, 2, 1, 1, 2, 2, 2, 2, 1};
-const bool kIsAns[NUM_OPS] = {false, false, false, false, false, false, false,
-                              true, true, true, true, true, true, true};
-
 int text_set_of(int op) {
   switch (op) {
     case OP_FIND: case OP_FILTER: return TS_FIND;
@@ -357,6 +353,24 @@ void build_waves(HostSchedule* out) {
       if (S.nodes[i].op != OP_FIND) S.wave_nodes[fill[S.depth[i]]++] = i;
   }
 
+}
+
+void build_bwd_order(HostSchedule* out) {
+  HostSchedule& W = *out;
+  // bucket 2*depth: the level's Transform nodes (the long CTAs: scheduled first), 2*depth + 1:
+  // its other nodes
+  const int nb = 2 * (W.max_depth + 1);
+  W.bwd_ptr.assign(nb + 1, 0);
+  auto bucket = [&](size_t i) { return 2 * W.depth[i] + (W.nodes[i].op == OP_TRANSFORM ? 0 : 1); };
+  for (size_t i = 0; i < W.nodes.size(); ++i) ++W.bwd_ptr[bucket(i) + 1];
+  for (int b = 0; b < nb; ++b) W.bwd_ptr[b + 1] += W.bwd_ptr[b];
+  W.bwd_nodes.assign(W.nodes.size(), 0);
+  std::vector<int32_t> fill(W.bwd_ptr.begin(), W.bwd_ptr.end() - 1);
+  for (size_t i = 0; i < W.nodes.size(); ++i) W.bwd_nodes[fill[bucket(i)]++] = (int32_t)i;
+  W.entry_order.resize(W.entries.size());
+  for (size_t i = 0; i < W.entries.size(); ++i) W.entry_order[i] = (int32_t)i;
+  std::stable_sort(W.entry_order.begin(), W.entry_order.end(),
+                   [&](int32_t a, int32_t b) { return W.entries[a].set < W.entries[b].set; });
 }
 
 // §8(d) traffic / work accounting; only needed when statistics are requested, so it is kept off

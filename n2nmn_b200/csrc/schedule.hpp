@@ -12,6 +12,11 @@
 
 namespace n2nmn {
 
+// Per opcode: attention inputs, and whether the module answers (ends a question).
+inline constexpr int kArity[NUM_OPS] = {0, 0, 1, 1, 1, 2, 2, 1, 1, 2, 2, 2, 2, 1};
+inline constexpr bool kIsAns[NUM_OPS] = {false, false, false, false, false, false, false,
+                                         true, true, true, true, true, true, true};
+
 struct SchedShape {
   int family, H, W, Dk, Dt, M, Mp, C, ksize;
   int max_T;
@@ -45,7 +50,7 @@ struct HostSchedule {
   int max_stack = 0;                  // most attention maps of one question alive at once
   std::vector<int32_t> wave_ptr;      // [max_depth+2], wave d = [wave_ptr[d], wave_ptr[d+1])
   std::vector<int32_t> wave_nodes;
-  std::vector<int32_t> bwd_ptr, bwd_nodes;   // training: ALL nodes bucketed by depth (capi.cu)
+  std::vector<int32_t> bwd_ptr, bwd_nodes;   // training: ALL nodes bucketed by depth (build_bwd_order)
   std::vector<int32_t> entry_order;          // training: B-map entries sorted by weight set
   // training schedules only: one [HW,Mp] gradient map per feature-side layer use
   bool train = false;
@@ -97,6 +102,10 @@ int finalize_schedule(const SchedShape& shp, int images_per_seg, HostSchedule* o
 
 // Fills wave_ptr / wave_nodes (depth-bucketed waves). Idempotent.
 void build_waves(HostSchedule* out);
+
+// Fills bwd_ptr / bwd_nodes and entry_order of a training schedule: every node bucketed by depth
+// (leaves = 1), since the backward runs one launch per level, top down.
+void build_bwd_order(HostSchedule* out);
 
 // Fills kbytes / kflops / per_node_* (SURVEY.md §8d). Idempotent.
 void account_schedule(const SchedShape& shp, HostSchedule* out);

@@ -34,6 +34,7 @@
 #include <vector>
 
 #include "../../include/n2nmn_b200.h"
+#include "launch.cuh"
 #include "mma_tile.cuh"
 
 namespace n2nmn {
@@ -508,19 +509,7 @@ struct n2nmn_seq2seq {
 
 namespace {
 
-template <class... KArgs, class... Args>
-cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                       cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t lc;
-  std::memset(&lc, 0, sizeof(lc));
-  lc.gridDim = grid; lc.blockDim = block; lc.dynamicSmemBytes = smem; lc.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  lc.attrs = attr;
-  lc.numAttrs = 1;
-  return cudaLaunchKernelEx(&lc, kernel, KArgs(args)...);
-}
+constexpr LaunchAttrs kPdl{true};
 
 // 32-row tiles while 64-row tiles would leave SMs without a CTA
 bool narrow_tiles(int col_blocks, int R, int num_sms) {
@@ -537,11 +526,11 @@ int launch_gemm(n2nmn_seq2seq* s, cudaStream_t st, const float* A, int lda, int 
   const bool exact = !(s->cfg.flags & N2NMN_SEQ2SEQ_FLAG_TF32) || force_exact;
   const dim3 gn(cb, (R + 31) / 32), gw(cb, (R + 63) / 64), blk(kMmaThreads);
   if (narrow_tiles(cb, R, s->num_sms)) {
-    if (exact) S2S_TRY(launch_pdl(s2s_gemm_kernel<2, true>, gn, blk, mma_smem_bytes(2), st, op, bias, out, ldo));
-    else S2S_TRY(launch_pdl(s2s_gemm_kernel<2, false>, gn, blk, mma_smem_bytes(2), st, op, bias, out, ldo));
+    if (exact) S2S_TRY(launch(s2s_gemm_kernel<2, true>, gn, blk, mma_smem_bytes(2), st, kPdl, op, bias, out, ldo));
+    else S2S_TRY(launch(s2s_gemm_kernel<2, false>, gn, blk, mma_smem_bytes(2), st, kPdl, op, bias, out, ldo));
   } else {
-    if (exact) S2S_TRY(launch_pdl(s2s_gemm_kernel<4, true>, gw, blk, mma_smem_bytes(4), st, op, bias, out, ldo));
-    else S2S_TRY(launch_pdl(s2s_gemm_kernel<4, false>, gw, blk, mma_smem_bytes(4), st, op, bias, out, ldo));
+    if (exact) S2S_TRY(launch(s2s_gemm_kernel<4, true>, gw, blk, mma_smem_bytes(4), st, kPdl, op, bias, out, ldo));
+    else S2S_TRY(launch(s2s_gemm_kernel<4, false>, gw, blk, mma_smem_bytes(4), st, kPdl, op, bias, out, ldo));
   }
   ++s->launches;
   return N2NMN_OK;
@@ -800,14 +789,14 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     const dim3 g3(grid.x, grid.y, nz), blk(kMmaThreads);
     cudaError_t le;
     if (!narrow) {
-      le = exact ? launch_pdl(lstm_step_kernel<4, true, 3>, g3, blk, mma_smem_bytes(4, 3), st, w)
-                 : launch_pdl(lstm_step_kernel<4, false, 3>, g3, blk, mma_smem_bytes(4, 3), st, w);
+      le = exact ? launch(lstm_step_kernel<4, true, 3>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w)
+                 : launch(lstm_step_kernel<4, false, 3>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w);
     } else if (shared_sm) {
-      le = exact ? launch_pdl(lstm_step_kernel<2, true, 3>, g3, blk, mma_smem_bytes(2, 3), st, w)
-                 : launch_pdl(lstm_step_kernel<2, false, 3>, g3, blk, mma_smem_bytes(2, 3), st, w);
+      le = exact ? launch(lstm_step_kernel<2, true, 3>, g3, blk, mma_smem_bytes(2, 3), st, kPdl, w)
+                 : launch(lstm_step_kernel<2, false, 3>, g3, blk, mma_smem_bytes(2, 3), st, kPdl, w);
     } else {
-      le = exact ? launch_pdl(lstm_step_kernel<2, true, 5>, g3, blk, mma_smem_bytes(2, 5), st, w)
-                 : launch_pdl(lstm_step_kernel<2, false, 5>, g3, blk, mma_smem_bytes(2, 5), st, w);
+      le = exact ? launch(lstm_step_kernel<2, true, 5>, g3, blk, mma_smem_bytes(2, 5), st, kPdl, w)
+                 : launch(lstm_step_kernel<2, false, 5>, g3, blk, mma_smem_bytes(2, 5), st, kPdl, w);
     }
     if (le != cudaSuccess) ok = false;
     ++s->launches;
@@ -859,7 +848,7 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     a.neg_entropy = neg_entropy_dev;
     a.atts = atts + (size_t)t * T_enc * N;
     a.T = T_enc; a.N = N; a.L = L; a.V = Vn;
-    if (launch_pdl(dec_attn_kernel, dim3(N), dim3(kAttnThreads), attn_smem, st, a) != cudaSuccess)
+    if (launch(dec_attn_kernel, dim3(N), dim3(kAttnThreads), attn_smem, st, kPdl, a) != cudaSuccess)
       ok = false;
     ++s->launches;
   }

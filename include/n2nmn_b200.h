@@ -385,8 +385,9 @@ int64_t n2nmn_launch_count(const n2nmn_ctx* ctx);
  * Replaces `AttentionSeq2Seq` (models_clevr/nmn3_netgen_att.py:46-322; the VQA / SHAPES copies
  * are the same code) without dropout: greedy decoding under the Assembler's validity masks,
  * `decoder_sampling` (n2nmn_seq2seq_set_sampling) or teacher forcing: the encoder LSTM stack
- * under dynamic_rnn (:73-120) and the raw_rnn attention decoder (:122-322). The backward pass is
- * not provided. */
+ * under dynamic_rnn (:73-120) and the raw_rnn attention decoder (:122-322). Training: a recording
+ * forward (n2nmn_seq2seq_set_record), n2nmn_seq2seq_backward into a flat gradient buffer and
+ * n2nmn_seq2seq_adam_step (DESIGN.md §4c). */
 typedef struct n2nmn_seq2seq n2nmn_seq2seq;
 typedef struct n2nmn_seq2seq_config {
   int32_t abi_version;     /* N2NMN_ABI_VERSION */
@@ -446,6 +447,39 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
  * token if it is invalid (:241-256). NULL = back to greedy decoding. gt_layout_dev still wins. */
 int n2nmn_seq2seq_set_sampling(n2nmn_seq2seq* s, const float* uniforms_dev);
 int64_t n2nmn_seq2seq_launch_count(const n2nmn_seq2seq* s);
+/* Recording switch for the following forward calls (default off). While on, the forward also
+ * keeps what n2nmn_seq2seq_backward needs: every cell's gates and state, every decoding step's
+ * attention query, context vector, token scores, validity mask and token, and a copy of the
+ * inputs. The workspace (~100 MB at N=64, T_enc=45, T_dec=10, lstm_dim=512, 2 layers) is
+ * allocated on first use. The outputs are bit-identical with and without recording. */
+int n2nmn_seq2seq_set_record(n2nmn_seq2seq* s, int on);
+/* Flat layout of the variables (creation order, n2nmn_seq2seq_variable_info), each in its TF shape
+ * and layout at a 16-byte aligned offset: the gradient, weight and Adam moment buffers. */
+int64_t n2nmn_seq2seq_flat_size(const n2nmn_seq2seq* s);
+int n2nmn_seq2seq_flat_offset(const n2nmn_seq2seq* s, int index, int64_t* offset, int64_t* count);
+/* Gradient of the generator's variables, after a recording forward of this batch, as TF 1.0
+ * differentiates nmn3_netgen_att.py's graph. Each upstream gradient may be NULL (= zero):
+ *   d_log_seq_prob_dev [N]              d total / d log_seq_prob (Σ_t log token_probs, nmn3_model.py:46)
+ *   d_neg_entropy_dev  [N]              d total / d neg_entropy
+ *   d_word_vecs_dev    [T_dec][N][E_txt] d total / d word_vecs
+ * with N the recorded forward's batch. No gradient flows through the validity masks, the decoding
+ * state or the chosen tokens. grad_flat_dev (n2nmn_seq2seq_flat_size floats) is overwritten.
+ * N2NMN_ERR_STATE if the last forward did not record or a weight was set since. All work is
+ * enqueued on `stream`; nothing is read back. */
+int n2nmn_seq2seq_backward(n2nmn_seq2seq* s, const float* d_log_seq_prob_dev,
+                           const float* d_neg_entropy_dev, const float* d_word_vecs_dev,
+                           float* grad_flat_dev, void* stream);
+/* All variables from / to one flat buffer (device, n2nmn_seq2seq_flat_offset layout). Loading
+ * marks the derived weights for re-preparation at the next forward. */
+int n2nmn_seq2seq_load_flat_weights(n2nmn_seq2seq* s, const float* wflat_dev, void* stream);
+int n2nmn_seq2seq_get_flat_weights(const n2nmn_seq2seq* s, float* wflat_dev, void* stream);
+/* One optimiser step over the flat buffers, as n2nmn_adam_step: g += weight_decay·w on every
+ * ".../weights" variable (the reference's l2_reg, nmn3_model.py:161-166), tf.clip_by_norm per
+ * tensor to max_norm, Adam with TF's lr_t; then the context takes the new weights
+ * (n2nmn_seq2seq_load_flat_weights). gflat_dev is modified (decay term). */
+int n2nmn_seq2seq_adam_step(n2nmn_seq2seq* s, float* wflat_dev, float* gflat_dev, float* m_dev,
+                            float* v_dev, int step, float lr, float beta1, float beta2, float eps,
+                            float max_norm, float weight_decay, void* stream);
 
 #ifdef __cplusplus
 }

@@ -52,6 +52,14 @@ SIGNATURES = {
     'n2nmn_seq2seq_forward': (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
     'n2nmn_seq2seq_set_sampling': (C.c_int, [_P, _P]),
     'n2nmn_seq2seq_launch_count': (C.c_int64, [_P]),
+    'n2nmn_seq2seq_set_record': (C.c_int, [_P, C.c_int]),
+    'n2nmn_seq2seq_backward': (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    'n2nmn_seq2seq_flat_size': (C.c_int64, [_P]),
+    'n2nmn_seq2seq_flat_offset': (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    'n2nmn_seq2seq_load_flat_weights': (C.c_int, [_P, _P, _P]),
+    'n2nmn_seq2seq_get_flat_weights': (C.c_int, [_P, _P, _P]),
+    'n2nmn_seq2seq_adam_step': (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_float,
+                                          C.c_float, C.c_float, C.c_float, _P]),
     'n2nmn_create': (C.c_int, [C.POINTER(Config), C.POINTER(_P)]),
     'n2nmn_destroy': (C.c_int, [_P]),
     'n2nmn_last_error': (C.c_char_p, []),

@@ -1748,7 +1748,7 @@ int adam_impl(n2nmn_ctx* c, float* wflat, float* gflat, float* m, float* v, int 
   const double lr_t = (double)lr * std::sqrt(1.0 - std::pow((double)beta2, step)) /
                       (1.0 - std::pow((double)beta1, step));
   TRY(ensure_repack_tables(c));
-  TRY(ctx_launch(c, adam_clip_kernel, grid, 256, 0, st, {}, wflat, gflat, m, v,
+  TRY(ctx_launch(c, adam_clip_kernel<true>, grid, 256, 0, st, {}, wflat, gflat, m, v,
                  c->d_segs, c->d_sumsq, (float)lr_t, beta1, beta2, eps, max_norm,
                  c->d_repack, c->wbuf, c->Mp));
   prof_mark(c, "clip_adam_kernels", st);

@@ -4,6 +4,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "optim.cuh"
 
 namespace n2nmn {
 
@@ -56,8 +57,8 @@ __global__ void widen_f16_kernel(const uint4* __restrict__ src, float4* __restri
 }
 
 // ---- all variables from one flat buffer in two launches (after every optimiser step) ------------
-// kind 0: plain copy of `count` floats; kind 1: [rows][cols] -> [rows][pitch] zero padded.
-struct RepackSeg { int src_off, count, cols, kind; long long dst_off; };
+// RepackSeg (optim.cuh) kind 0: plain copy of `count` floats; kind 1: [rows][cols] -> [rows][pitch]
+// zero padded.
 // grid = (16, variables)
 __global__ void repack_all_kernel(const float* __restrict__ wflat, const RepackSeg* __restrict__ segs,
                                   float* __restrict__ wbuf, int pitch) {

@@ -26,9 +26,13 @@
 // (weights, tables) before griddepcontrol.wait.
 // At N = 64 an LSTM launch costs the issue time of its mma.sync instructions (three passes for fp32
 // parity; DESIGN.md §4c).
+// Training: with n2nmn_seq2seq_set_record on, the forward also stores what the backward pass
+// (n2nmn_seq2seq_backward, kernels in seq2seq_bwd.cuh) reads; n2nmn_seq2seq_adam_step runs the
+// module network's clip + Adam kernels (optim.cuh) over the flat variable layout.
 #include <cuda_runtime.h>
 
 #include <cmath>
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -36,6 +40,7 @@
 #include "../../include/n2nmn_b200.h"
 #include "launch.cuh"
 #include "mma_tile.cuh"
+#include "optim.cuh"
 
 namespace n2nmn {
 int fail_with(int code, const std::string& msg);   // capi.cu: sets n2nmn_last_error()
@@ -117,6 +122,9 @@ struct LstmStep {
   float* out_seq;        // encoder top layer: encoder_outputs[t] (zero past the end) or nullptr
   const int32_t* seq_len;   // encoder: [N]; nullptr in the decoder (every row live)
   int t, N, L;
+  // recording forward only (kRecord): activated gates i, j, f, o [N][4L] in TF's column order,
+  // c_t and h_t [N][L] (the carried state past the sequence end)
+  float *rec_gates, *rec_c, *rec_h;
 };
 
 // BasicLSTMCell(forget_bias=1) step (gate order i, j, f, o) with dynamic_rnn's masking: past the
@@ -129,7 +137,7 @@ struct LstmStep {
 // 3-stage ring two CTAs share an SM, which keeps as many bytes in flight as the 5-stage ring of
 // the single-step launches.
 struct LstmWave { LstmStep s[kMaxLayers]; };
-template <int WM, bool kExact, int ST>
+template <int WM, bool kExact, int ST, bool kRecord = false>
 __global__ void __launch_bounds__(kMmaThreads) lstm_step_kernel(const LstmWave wave) {
   pdl_trigger();
   const LstmStep& p = wave.s[blockIdx.z];
@@ -196,6 +204,24 @@ __global__ void __launch_bounds__(kMmaThreads) lstm_step_kernel(const LstmWave w
     *reinterpret_cast<float2*>(p.h_out + idx) = make_float2(h_new[0], h_new[1]);
     if (p.out_seq != nullptr)
       *reinterpret_cast<float2*>(p.out_seq + idx) = make_float2(o_new[0], o_new[1]);
+    if constexpr (kRecord) {
+      const size_t gi0 = (size_t)n * C + (c0 >> 2) + 2 * tig;
+      float2 act[4];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const float a0 = sigmoidf_(gt[hh][0][j] + acc[0][hh * 2 + j]);
+        const float a1 = tanhf(gt[hh][1][j] + acc[1][hh * 2 + j]);
+        const float a2 = sigmoidf_(gt[hh][2][j] + acc[2][hh * 2 + j] + 1.0f);
+        const float a3 = sigmoidf_(gt[hh][3][j] + acc[3][hh * 2 + j]);
+        (j == 0 ? act[0].x : act[0].y) = a0; (j == 0 ? act[1].x : act[1].y) = a1;
+        (j == 0 ? act[2].x : act[2].y) = a2; (j == 0 ? act[3].x : act[3].y) = a3;
+      }
+#pragma unroll
+      for (int gate = 0; gate < 4; ++gate)
+        *reinterpret_cast<float2*>(p.rec_gates + gi0 + (size_t)gate * L) = act[gate];
+      *reinterpret_cast<float2*>(p.rec_c + idx) = make_float2(c_new[0], c_new[1]);
+      *reinterpret_cast<float2*>(p.rec_h + idx) = make_float2(h_new[0], h_new[1]);
+    }
   }
 }
 
@@ -220,6 +246,10 @@ struct AttnStep {
   float* neg_entropy;     // [N] accumulated
   float* atts;            // [T][N] this step's attention
   int T, N, L, V;
+  // recording forward only (kRecord): context vector [N][L], token scores [N][V], validity bits
+  // [N][2], attention [T][N], chosen token [N]
+  float *rec_d2, *rec_sc, *rec_att;
+  int32_t *rec_valid, *rec_tok;
 };
 
 // One CTA per question: nmn3_netgen_att.py:205-293 for one decoding step. Everything that does
@@ -232,6 +262,7 @@ __host__ __device__ inline size_t attn_smem_floats(int L, int T, int V) {
   return (size_t)V * 2 * L + 4 * L + part + ((T + 3) & ~3) + 2 * ((V + 3) & ~3) + 3 * V + 12 * V +
          4 * V + 8;
 }
+template <bool kRecord = false>
 __global__ void __launch_bounds__(kAttnThreads) dec_attn_kernel(AttnStep p) {
   pdl_trigger();
   extern __shared__ __align__(16) float sm[];
@@ -313,6 +344,7 @@ __global__ void __launch_bounds__(kAttnThreads) dec_attn_kernel(AttnStep p) {
       const float a = s_att[te] / s2;
       s_att[te] = a;
       p.atts[(size_t)te * p.N + n] = a;
+      if constexpr (kRecord) p.rec_att[(size_t)te * p.N + n] = a;
     }
   } else if (warp == 1) {
     // validity of every token from the decoding state (:8-11); all ones under forcing (:230-233)
@@ -333,6 +365,8 @@ __global__ void __launch_bounds__(kAttnThreads) dec_attn_kernel(AttnStep p) {
       if (base == 0) lo = bal; else hi = bal;
     }
     if (lane == 0) { s_valid[0] = (int32_t)lo; s_valid[1] = (int32_t)hi; }
+    if constexpr (kRecord)
+      if (lane == 0) { p.rec_valid[2 * n] = (int32_t)lo; p.rec_valid[2 * n + 1] = (int32_t)hi; }
   }
   __syncthreads();
   // d2 = Σ_te att[te] encoder_outputs[te]   (:218): G groups of threads split the time steps of
@@ -356,6 +390,7 @@ __global__ void __launch_bounds__(kAttnThreads) dec_attn_kernel(AttnStep p) {
       float s = 0.f;
       for (int gi = 0; gi < G; ++gi) s += s_part[(size_t)gi * L + d];
       s_x[L + d] = s;
+      if constexpr (kRecord) p.rec_d2[(size_t)n * L + d] = s;
     }
   }
   tp_wait<0>();
@@ -371,6 +406,8 @@ __global__ void __launch_bounds__(kAttnThreads) dec_attn_kernel(AttnStep p) {
 #pragma unroll
     for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     if (lane == 0) s_sc[vv] = s + s_by[vv];
+    if constexpr (kRecord)
+      if (lane == 0) p.rec_sc[(size_t)n * V + vv] = s + s_by[vv];
   }
   __syncthreads();
   if (warp == 0) {   // lane handles tokens lane and lane + 32 (V <= 64)
@@ -440,6 +477,7 @@ __global__ void __launch_bounds__(kAttnThreads) dec_attn_kernel(AttnStep p) {
       p.X[n * 3 + 2] += s_P[pred * 3 + 2];
       p.tokens[n] = pred;
       p.cur_tok[n] = pred;
+      if constexpr (kRecord) p.rec_tok[n] = pred;
     }
   }
 }
@@ -476,12 +514,15 @@ __global__ void init_state_kernel(int32_t* X, int32_t* cur_tok, float* neg_entro
 struct S2SVar {
   std::string name;
   std::vector<int64_t> shape;
-  float* dev;       // raw copy as given (TF layout)
+  float* dev;       // raw copy as given (TF layout), inside the context's flat variable buffer
   size_t count;
+  int64_t offset;   // in the flat layout (16-byte aligned)
   bool loaded;
 };
 
 }  // namespace
+
+#include "seq2seq_bwd.cuh"
 
 struct n2nmn_seq2seq {
   n2nmn_seq2seq_config cfg;
@@ -500,6 +541,29 @@ struct n2nmn_seq2seq {
   float *enc_out = nullptr, *enc_ht = nullptr, *q = nullptr, *atts = nullptr;
   int32_t *X = nullptr, *cur_tok = nullptr, *P = nullptr, *W = nullptr, *b = nullptr;
   int64_t launches = 0;
+  float* wstore = nullptr;   // every variable, flat layout (n2nmn_seq2seq_flat_offset)
+  int64_t flat_size = 0;
+  // recording forward (n2nmn_seq2seq_set_record): what the backward pass reads. Slots are sized
+  // for max_batch and T_encoder; inside a (side, layer) block the rows are [t][N] with the
+  // recorded N, so that all steps of a layer form one [T·N] matrix.
+  bool record = false;
+  bool rec_ready = false;    // workspace allocated (all of it)
+  bool rec_valid = false;    // the last forward recorded and no weight changed since
+  int rec_N = 0, rec_T = 0;
+  float *rec_gates[2] = {}, *rec_c[2] = {}, *rec_h[2] = {};   // [layers][T_cap][N][4L | L]
+  float *rec_q = nullptr, *rec_d2 = nullptr, *rec_sc = nullptr, *rec_att = nullptr;
+  int32_t *rec_valid_bits = nullptr, *rec_tok = nullptr, *rec_seq = nullptr, *rec_len = nullptr;
+  // backward workspace, allocated with the recording
+  float *dgates[2] = {};     // [layers][T_cap][N][4L]
+  float *d_h[4] = {};        // drec, dup, hcarry, dc: [layers][N][L] each
+  float *ds = nullptr, *dh_top = nullptr, *dq = nullptr, *dv_part = nullptr;
+  float *d_enc_out = nullptr, *d_enc_ht = nullptr, *dx0 = nullptr;
+  float *w_t[2][kMaxLayers] = {};   // transposed cell matrices [4L][in + L] (TF layout)
+  float *wa_t = nullptr, *wh_t = nullptr;
+  bool bwd_dirty = true;     // transposes stale
+  VarSeg* d_segs = nullptr;  // Adam segment table, ready with d_sumsq
+  float* d_sumsq = nullptr;
+  bool segs_ready = false;
   int var(const std::string& n) const {
     for (size_t i = 0; i < vars.size(); ++i) if (vars[i].name == n) return (int)i;
     return -1;
@@ -579,6 +643,324 @@ int prepare(n2nmn_seq2seq* s, cudaStream_t st) {
 
 template <class T>
 cudaError_t dmalloc(T** p, size_t n) { return cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)); }
+template <class T>
+cudaError_t dmalloc_once(T** p, size_t n) { return *p ? cudaSuccess : dmalloc(p, n); }
+
+int t_cap(const n2nmn_seq2seq* s, int side) { return side == 0 ? s->cfg.T_encoder : s->cfg.T_decoder; }
+// recorded rows of (side, layer) from step t on, with the recorded batch size N
+float* rec_gates_at(n2nmn_seq2seq* s, int side, int l, int t, int N) {
+  const size_t L4 = 4 * (size_t)s->cfg.lstm_dim;
+  return s->rec_gates[side] + ((size_t)l * t_cap(s, side) * s->cfg.max_batch + (size_t)t * N) * L4;
+}
+float* dgates_at(n2nmn_seq2seq* s, int side, int l, int t, int N) {
+  const size_t L4 = 4 * (size_t)s->cfg.lstm_dim;
+  return s->dgates[side] + ((size_t)l * t_cap(s, side) * s->cfg.max_batch + (size_t)t * N) * L4;
+}
+float* rec_state_at(n2nmn_seq2seq* s, float* base, int side, int l, int t, int N) {
+  const size_t L = s->cfg.lstm_dim;
+  return base + ((size_t)l * t_cap(s, side) * s->cfg.max_batch + (size_t)t * N) * L;
+}
+
+// The recording and backward workspace, allocated on first use. Ready only when all of it is:
+// a failed attempt leaves rec_ready false and the next call allocates what is still missing.
+int ensure_record(n2nmn_seq2seq* s) {
+  if (s->rec_ready) return N2NMN_OK;
+  const auto& g = s->cfg;
+  const size_t L = g.lstm_dim, N = g.max_batch, NL = g.num_layers, Td = g.T_decoder;
+  const size_t Te = g.T_encoder, Vn = g.num_vocab_nmn, Vp = (Vn + 3) & ~size_t(3);
+  for (int side = 0; side < 2; ++side) {
+    const size_t rows = NL * (size_t)t_cap(s, side) * N;
+    S2S_TRY(dmalloc_once(&s->rec_gates[side], rows * 4 * L));
+    S2S_TRY(dmalloc_once(&s->rec_c[side], rows * L));
+    S2S_TRY(dmalloc_once(&s->rec_h[side], rows * L));
+    S2S_TRY(dmalloc_once(&s->dgates[side], rows * 4 * L));
+    for (size_t l = 0; l < NL; ++l) {
+      const size_t in = l == 0 ? (side == 0 ? g.embed_dim_txt : g.embed_dim_nmn) : L;
+      S2S_TRY(dmalloc_once(&s->w_t[side][l], 4 * L * (in + L)));
+    }
+  }
+  S2S_TRY(dmalloc_once(&s->rec_q, Td * N * L));
+  S2S_TRY(dmalloc_once(&s->rec_d2, Td * N * L));
+  S2S_TRY(dmalloc_once(&s->rec_sc, Td * N * Vn));
+  S2S_TRY(dmalloc_once(&s->rec_att, Td * Te * N));
+  S2S_TRY(dmalloc_once(&s->rec_valid_bits, Td * N * 2));
+  S2S_TRY(dmalloc_once(&s->rec_tok, Td * N));
+  S2S_TRY(dmalloc_once(&s->rec_seq, Te * N));
+  S2S_TRY(dmalloc_once(&s->rec_len, N));
+  for (auto*& p : s->d_h) S2S_TRY(dmalloc_once(&p, NL * N * L));
+  S2S_TRY(dmalloc_once(&s->ds, Td * N * Vp));
+  S2S_TRY(dmalloc_once(&s->dh_top, Td * N * L));
+  S2S_TRY(dmalloc_once(&s->dq, Td * N * L));
+  S2S_TRY(dmalloc_once(&s->dv_part, N * L));
+  S2S_TRY(dmalloc_once(&s->d_enc_out, Te * N * L));
+  S2S_TRY(dmalloc_once(&s->d_enc_ht, Te * N * L));
+  const size_t E = std::max(g.embed_dim_txt * Te, g.embed_dim_nmn * Td);
+  S2S_TRY(dmalloc_once(&s->dx0, E * N));
+  S2S_TRY(dmalloc_once(&s->wa_t, L * L));
+  S2S_TRY(dmalloc_once(&s->wh_t, L * L));
+  auto opt_in = [](auto kernel, size_t bytes) {
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  };
+  S2S_TRY(opt_in(lstm_step_kernel<2, true, 5, true>, mma_smem_bytes(2, 5)));
+  S2S_TRY(opt_in(lstm_step_kernel<2, false, 5, true>, mma_smem_bytes(2, 5)));
+  S2S_TRY(opt_in(lstm_step_kernel<2, true, 3, true>, mma_smem_bytes(2, 3)));
+  S2S_TRY(opt_in(lstm_step_kernel<2, false, 3, true>, mma_smem_bytes(2, 3)));
+  S2S_TRY(opt_in(lstm_step_kernel<4, true, 3, true>, mma_smem_bytes(4, 3)));
+  S2S_TRY(opt_in(lstm_step_kernel<4, false, 3, true>, mma_smem_bytes(4, 3)));
+  S2S_TRY(cudaFuncSetAttribute(lstm_step_kernel<2, true, 3, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+  S2S_TRY(cudaFuncSetAttribute(lstm_step_kernel<2, false, 3, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+  S2S_TRY(opt_in(dec_attn_kernel<true>, attn_smem_floats(g.lstm_dim, g.T_encoder, Vn) * sizeof(float)));
+  S2S_TRY(opt_in(s2s_bwd_gemm_kernel<2, true>, mma_smem_bytes(2)));
+  S2S_TRY(opt_in(s2s_bwd_gemm_kernel<2, false>, mma_smem_bytes(2)));
+  S2S_TRY(opt_in(s2s_bwd_gemm_kernel<4, true>, mma_smem_bytes(4)));
+  S2S_TRY(opt_in(s2s_bwd_gemm_kernel<4, false>, mma_smem_bytes(4)));
+  S2S_TRY(opt_in(s2s_head_bwd_kernel, head_bwd_smem_floats(g.lstm_dim, g.T_encoder) * sizeof(float)));
+  s->rec_ready = true;
+  return N2NMN_OK;
+}
+
+// ---- backward helpers ---------------------------------------------------------------------------
+// The transposed matrices of the backward products, re-made after a weight changed.
+int prepare_backward(n2nmn_seq2seq* s, cudaStream_t st) {
+  const auto& g = s->cfg;
+  const int L = g.lstm_dim;
+  for (int side = 0; side < 2; ++side)
+    for (int l = 0; l < g.num_layers; ++l) {
+      const int in = l == 0 ? (side == 0 ? g.embed_dim_txt : g.embed_dim_nmn) : L;
+      transpose_kernel<<<s->num_sms, 256, 0, st>>>(s->v(cell_prefix(side, l) + "weights"),
+                                                   s->w_t[side][l], in + L, 4 * L);
+      ++s->launches;
+    }
+  transpose_kernel<<<64, 256, 0, st>>>(s->v("decoder/att_prediction/weights"), s->wa_t, L, L);
+  transpose_kernel<<<64, 256, 0, st>>>(s->v("encoder/encoder_h_transform/weights"), s->wh_t, L, L);
+  s->launches += 2;
+  S2S_TRY(cudaGetLastError());
+  s->bwd_dirty = false;
+  return N2NMN_OK;
+}
+
+GemmOperands gemm_ops(const float* A, int lda, int R, int K, const float* B, int ldb, int C) {
+  GemmOperands op;
+  op.a0 = A; op.k0 = K; op.lda0 = lda; op.a1 = nullptr; op.k1 = 0; op.lda1 = 0;
+  op.R = R; op.B = B; op.ldb = ldb; op.C = C;
+  return op;
+}
+
+// One launch of s2s_bwd_gemm_kernel over `nz` slots; exact = the error-compensated 3xTF32 path.
+int launch_bwd_gemm(n2nmn_seq2seq* s, cudaStream_t st, const BwdGemmWave& w, int nz) {
+  int R = 0, C = 0;
+  for (int z = 0; z < nz; ++z) { R = std::max(R, w.s[z].op.R); C = std::max(C, w.s[z].op.C); }
+  const int cb = (C + kMmaCols - 1) / kMmaCols;
+  const bool exact = !(s->cfg.flags & N2NMN_SEQ2SEQ_FLAG_TF32);
+  const dim3 blk(kMmaThreads);
+  if (narrow_tiles(cb * nz, R, s->num_sms)) {
+    const dim3 grid(cb, (R + 31) / 32, nz);
+    S2S_TRY(exact ? launch(s2s_bwd_gemm_kernel<2, true>, grid, blk, mma_smem_bytes(2), st, kPdl, w)
+                  : launch(s2s_bwd_gemm_kernel<2, false>, grid, blk, mma_smem_bytes(2), st, kPdl, w));
+  } else {
+    const dim3 grid(cb, (R + 63) / 64, nz);
+    S2S_TRY(exact ? launch(s2s_bwd_gemm_kernel<4, true>, grid, blk, mma_smem_bytes(4), st, kPdl, w)
+                  : launch(s2s_bwd_gemm_kernel<4, false>, grid, blk, mma_smem_bytes(4), st, kPdl, w));
+  }
+  ++s->launches;
+  return N2NMN_OK;
+}
+
+BwdGemm bwd_gemm(GemmOperands op, float* out0, int ldo0, float* out1, int ldo1, int split,
+                 bool accumulate) {
+  BwdGemm b;
+  b.op = op; b.out0 = out0; b.ldo0 = ldo0; b.out1 = out1; b.ldo1 = ldo1; b.split = split;
+  b.accumulate = accumulate ? 1 : 0;
+  return b;
+}
+
+int one_gemm(n2nmn_seq2seq* s, cudaStream_t st, const BwdGemm& g) {
+  BwdGemmWave w;
+  std::memset(&w, 0, sizeof(w));
+  w.s[0] = g;
+  return launch_bwd_gemm(s, st, w, 1);
+}
+
+int launch_xtb(n2nmn_seq2seq* s, cudaStream_t st, const XtbSrc& x) {
+  const int K = x.kx + x.kh;
+  const dim3 grid0((x.C + kXtbTile - 1) / kXtbTile, (K + kXtbTile - 1) / kXtbTile);
+  const int tiles = grid0.x * grid0.y;
+  // split the rows while the tiles alone leave SMs idle, keeping >= 128 rows per split
+  int splits = std::max(1, std::min((2 * s->num_sms + tiles - 1) / tiles, x.R / 128));
+  s2s_xtb_kernel<<<dim3(grid0.x, grid0.y, splits), 256, 0, st>>>(x);
+  ++s->launches;
+  S2S_TRY(cudaGetLastError());
+  return N2NMN_OK;
+}
+
+int launch_colsum(n2nmn_seq2seq* s, cudaStream_t st, const float* in, int R, int ld, int C, float* out) {
+  const int cb = (C + 255) / 256;
+  const int splits = std::max(1, std::min((2 * s->num_sms + cb - 1) / cb, R / 64));
+  s2s_colsum_kernel<<<dim3(cb, splits), 256, 0, st>>>(in, R, ld, C, out);
+  ++s->launches;
+  S2S_TRY(cudaGetLastError());
+  return N2NMN_OK;
+}
+
+XtbSrc xtb_src() { XtbSrc x; std::memset(&x, 0, sizeof(x)); return x; }
+
+int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const float* dwv,
+                  float* gflat, cudaStream_t st) {
+  const auto& g = s->cfg;
+  const int L = g.lstm_dim, L4 = 4 * L, NL = g.num_layers, Vn = g.num_vocab_nmn;
+  const int Vp = (Vn + 3) & ~3, Et = g.embed_dim_txt, En = g.embed_dim_nmn, Td = g.T_decoder;
+  const int N = s->rec_N, T = s->rec_T;
+  auto off = [&](const std::string& name) { return gflat + s->vars[s->var(name)].offset; };
+  if (s->bwd_dirty) {
+    const int rc = prepare_backward(s, st);
+    if (rc) return rc;
+  }
+  S2S_TRY(cudaMemsetAsync(gflat, 0, sizeof(float) * s->flat_size, st));
+  for (auto* p : s->d_h) S2S_TRY(cudaMemsetAsync(p, 0, sizeof(float) * NL * g.max_batch * L, st));
+  S2S_TRY(cudaMemsetAsync(s->d_enc_out, 0, sizeof(float) * T * N * L, st));
+  S2S_TRY(cudaMemsetAsync(s->d_enc_ht, 0, sizeof(float) * T * N * L, st));
+  float *drec = s->d_h[0], *dup = s->d_h[1], *hcarry = s->d_h[2], *dc = s->d_h[3];
+  const size_t NLs = (size_t)g.max_batch * L;   // per-layer stride of the dh buffers
+  // ---- 1. decoder head, every step at once
+  HeadBwd hb;
+  hb.sc = s->rec_sc; hb.valid = s->rec_valid_bits; hb.tok = s->rec_tok; hb.att = s->rec_att;
+  hb.q = s->rec_q; hb.enc_ht = s->enc_ht; hb.enc_out = s->enc_out;
+  hb.emb_txt = s->v("encoder/embedding_mat"); hb.seq = s->rec_seq; hb.seq_len = s->rec_len;
+  hb.v = s->v("decoder/att_prediction/v"); hb.wy = s->v("decoder/token_prediction/weights");
+  hb.dlp = dlp; hb.dne = dne; hb.dwv = dwv;
+  hb.ds = s->ds; hb.dh_top = s->dh_top; hb.dq = s->dq; hb.d_enc_out = s->d_enc_out;
+  hb.d_enc_ht = s->d_enc_ht; hb.dv_part = s->dv_part; hb.d_emb_txt = off("encoder/embedding_mat");
+  hb.T = T; hb.N = N; hb.L = L; hb.V = Vn; hb.Vp = Vp; hb.Td = Td; hb.E = Et;
+  s2s_head_bwd_kernel<<<N, kHeadBwdThreads, head_bwd_smem_floats(L, T) * sizeof(float), st>>>(hb);
+  ++s->launches;
+  S2S_TRY(cudaGetLastError());
+  // dh_top += dq · W_aᵀ over all T_dec·N rows; att_prediction, token_prediction and v gradients
+  const int Rd = Td * N;
+  const float* h_top = rec_state_at(s, s->rec_h[1], 1, NL - 1, 0, N);   // [Td·N][L]
+  int rc = one_gemm(s, st, bwd_gemm(gemm_ops(s->dq, L, Rd, L, s->wa_t, L, L), s->dh_top, L,
+                                    nullptr, 0, L, true));
+  if (rc) return rc;
+  XtbSrc x = xtb_src();
+  x.x = h_top; x.ldx = L; x.kx = L; x.G = s->dq; x.ldg = L; x.C = L; x.R = Rd;
+  x.out = off("decoder/att_prediction/weights"); x.ldo = L;
+  if ((rc = launch_xtb(s, st, x))) return rc;
+  if ((rc = launch_colsum(s, st, s->dq, Rd, L, L, off("decoder/att_prediction/biases")))) return rc;
+  x = xtb_src();
+  x.x = h_top; x.ldx = L; x.kx = L; x.hb = s->rec_d2; x.ldh = L; x.kh = L;
+  x.G = s->ds; x.ldg = Vp; x.C = Vn; x.R = Rd;
+  x.out = off("decoder/token_prediction/weights"); x.ldo = Vn;
+  if ((rc = launch_xtb(s, st, x))) return rc;
+  if ((rc = launch_colsum(s, st, s->ds, Rd, Vp, Vn, off("decoder/token_prediction/biases")))) return rc;
+  if ((rc = launch_colsum(s, st, s->dv_part, N, L, L, off("decoder/att_prediction/v")))) return rc;
+  // ---- 2. decoder BPTT, one cell backward and one [dx, dh_prev] product per layer and step
+  auto in_dim = [&](int side, int l) { return l == 0 ? (side == 0 ? Et : En) : L; };
+  auto cell_slot = [&](int side, int l, int t) {
+    CellBwd c;
+    c.gates = rec_gates_at(s, side, l, t, N);
+    c.c_prev = t > 0 ? rec_state_at(s, s->rec_c[side], side, l, t - 1, N)
+                     : (side == 1 ? rec_state_at(s, s->rec_c[0], 0, l, T - 1, N) : nullptr);
+    c.c_new = rec_state_at(s, s->rec_c[side], side, l, t, N);
+    c.drec = drec + l * NLs;
+    c.dup = l < NL - 1 ? dup + l * NLs : nullptr;
+    c.dtop = l == NL - 1 ? (side == 1 ? s->dh_top : s->d_enc_out) + (size_t)t * N * L : nullptr;
+    c.hcarry = side == 0 ? hcarry + l * NLs : nullptr;
+    c.dc = dc + l * NLs;
+    c.dgates = dgates_at(s, side, l, t, N);
+    c.seq_len = side == 0 ? s->rec_len : nullptr;
+    c.t = t; c.N = N; c.L = L;
+    return c;
+  };
+  auto gemm_slot = [&](int side, int l, int t) {   // [dx, dh_prev] = dgates · Wᵀ (layer 0: dh only)
+    const int in = in_dim(side, l);
+    const float* B = s->w_t[side][l] + (l == 0 ? in : 0);
+    return bwd_gemm(gemm_ops(dgates_at(s, side, l, t, N), L4, N, L4, B, in + L, l == 0 ? L : in + L),
+                    l == 0 ? nullptr : dup + (l - 1) * NLs, L, drec + l * NLs, L, l == 0 ? 0 : in,
+                    false);
+  };
+  auto launch_cells = [&](const CellBwdWave& w, int nz) {
+    const dim3 grid((N * L + 255) / 256, 1, nz);
+    ++s->launches;
+    return launch(s2s_cell_bwd_kernel, grid, dim3(256), 0, st, kPdl, w);
+  };
+  for (int t = Td - 1; t >= 0; --t)
+    for (int l = NL - 1; l >= 0; --l) {
+      CellBwdWave cw;
+      std::memset(&cw, 0, sizeof(cw));
+      cw.s[0] = cell_slot(1, l, t);
+      S2S_TRY(launch_cells(cw, 1));
+      BwdGemmWave gw;
+      std::memset(&gw, 0, sizeof(gw));
+      gw.s[0] = gemm_slot(1, l, t);
+      if ((rc = launch_bwd_gemm(s, st, gw, 1))) return rc;
+    }
+  // ---- 3. encoder: d enc_out += d enc_ht · W_hᵀ, encoder_h_transform gradients
+  const int Re = T * N;
+  rc = one_gemm(s, st, bwd_gemm(gemm_ops(s->d_enc_ht, L, Re, L, s->wh_t, L, L), s->d_enc_out, L,
+                                nullptr, 0, L, true));
+  if (rc) return rc;
+  x = xtb_src();
+  x.x = s->enc_out; x.ldx = L; x.kx = L; x.G = s->d_enc_ht; x.ldg = L; x.C = L; x.R = Re;
+  x.out = off("encoder/encoder_h_transform/weights"); x.ldo = L;
+  if ((rc = launch_xtb(s, st, x))) return rc;
+  if ((rc = launch_colsum(s, st, s->d_enc_ht, Re, L, L, off("encoder/encoder_h_transform/biases"))))
+    return rc;
+  // reverse wavefront: tick k runs layer l at step t = T - 1 - k + (layers - 1 - l)
+  for (int k = 0; k < T + NL - 1; ++k) {
+    CellBwdWave cw;
+    BwdGemmWave gw;
+    std::memset(&cw, 0, sizeof(cw));
+    std::memset(&gw, 0, sizeof(gw));
+    for (int l = 0; l < NL; ++l) {
+      const int t = T - 1 - k + (NL - 1 - l);
+      if (t < 0 || t >= T) continue;   // idle slot (N = 0, R = 0)
+      cw.s[l] = cell_slot(0, l, t);
+      gw.s[l] = gemm_slot(0, l, t);
+    }
+    S2S_TRY(launch_cells(cw, NL));
+    if ((rc = launch_bwd_gemm(s, st, gw, NL))) return rc;
+  }
+  // ---- 4. cell weight and bias gradients over all steps; layer-0 input rows
+  for (int side = 0; side < 2; ++side) {
+    const int Ts = side == 0 ? T : Td, R = Ts * N;
+    for (int l = 0; l < NL; ++l) {
+      const int in = in_dim(side, l);
+      x = xtb_src();
+      if (l == 0) {
+        x.table = side == 0 ? s->v("encoder/embedding_mat") : s->dec_rows;
+        x.idx = side == 0 ? s->rec_seq : s->rec_tok;
+        x.shift = side == 0 ? 0 : N;   // decoder step 0 reads go_embedding (row V of dec_rows)
+        x.first_idx = Vn;
+      } else {
+        x.x = rec_state_at(s, s->rec_h[side], side, l - 1, 0, N); x.ldx = L;
+      }
+      x.kx = in;
+      x.h0 = side == 0 ? nullptr : rec_state_at(s, s->rec_h[0], 0, l, T - 1, N);
+      x.hb = rec_state_at(s, s->rec_h[side], side, l, 0, N);
+      x.h0_rows = N; x.ldh = L; x.kh = L;
+      x.G = dgates_at(s, side, l, 0, N); x.ldg = L4; x.C = L4; x.R = R;
+      x.out = off(cell_prefix(side, l) + "weights"); x.ldo = L4;
+      if ((rc = launch_xtb(s, st, x))) return rc;
+      if ((rc = launch_colsum(s, st, dgates_at(s, side, l, 0, N), R, L4, L4,
+                              off(cell_prefix(side, l) + "biases"))))
+        return rc;
+    }
+    // embedding rows: d x0 = dgates · W_xᵀ, scattered into the looked-up rows
+    rc = one_gemm(s, st, bwd_gemm(gemm_ops(dgates_at(s, side, 0, 0, N), L4, R, L4, s->w_t[side][0],
+                                           in_dim(side, 0) + L, in_dim(side, 0)),
+                                  s->dx0, in_dim(side, 0), nullptr, 0, in_dim(side, 0), false));
+    if (rc) return rc;
+    if (side == 0)
+      s2s_scatter_rows_kernel<<<R, 128, 0, st>>>(s->dx0, Et, s->rec_seq, 0, 0,
+                                                  off("encoder/embedding_mat"), g.num_vocab_txt, nullptr);
+    else
+      s2s_scatter_rows_kernel<<<R, 128, 0, st>>>(s->dx0, En, s->rec_tok, N, Vn,
+                                                  off("decoder/embedding_mat"), Vn,
+                                                  off("decoder/go_embedding"));
+    ++s->launches;
+    S2S_TRY(cudaGetLastError());
+  }
+  return N2NMN_OK;
+}
 
 }  // namespace
 
@@ -631,7 +1013,13 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
     add(cell_prefix(1, l) + "weights", {(l == 0 ? En : L) + L, C});
     add(cell_prefix(1, l) + "biases", {C});
   }
-  for (auto& v : s->vars) S2S_TRY(dmalloc(&v.dev, v.count));
+  for (auto& v : s->vars) {
+    v.offset = s->flat_size;
+    s->flat_size += (int64_t)((v.count + 3) & ~size_t(3));
+  }
+  S2S_TRY(dmalloc(&s->wstore, (size_t)s->flat_size));
+  S2S_TRY(cudaMemset(s->wstore, 0, sizeof(float) * s->flat_size));
+  for (auto& v : s->vars) v.dev = s->wstore + v.offset;
   S2S_TRY(dmalloc(&s->table_enc, (size_t)Vt * C));
   S2S_TRY(dmalloc(&s->table_dec, (size_t)(Vn + 1) * C));
   S2S_TRY(dmalloc(&s->dec_rows, (size_t)(Vn + 1) * En));
@@ -675,7 +1063,7 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
   const size_t attn_bytes = attn_smem_floats(L, cfg->T_encoder, Vn) * sizeof(float);
   if (attn_bytes > 200 * 1024)
     return fail_with(N2NMN_ERR_ARG, "num_vocab_nmn * lstm_dim too large for the decoder step kernel");
-  S2S_TRY(cudaFuncSetAttribute(dec_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  S2S_TRY(cudaFuncSetAttribute(dec_attn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)attn_bytes));
   *out = s;
   return N2NMN_OK;
@@ -683,7 +1071,18 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
 
 int n2nmn_seq2seq_destroy(n2nmn_seq2seq* s) {
   if (!s) return N2NMN_OK;
-  for (auto& v : s->vars) cudaFree(v.dev);
+  cudaFree(s->wstore);
+  for (int side = 0; side < 2; ++side) {
+    cudaFree(s->rec_gates[side]); cudaFree(s->rec_c[side]); cudaFree(s->rec_h[side]);
+    cudaFree(s->dgates[side]);
+    for (int l = 0; l < kMaxLayers; ++l) cudaFree(s->w_t[side][l]);
+  }
+  cudaFree(s->rec_q); cudaFree(s->rec_d2); cudaFree(s->rec_sc); cudaFree(s->rec_att);
+  cudaFree(s->rec_valid_bits); cudaFree(s->rec_tok); cudaFree(s->rec_seq); cudaFree(s->rec_len);
+  for (auto* p : s->d_h) cudaFree(p);
+  cudaFree(s->ds); cudaFree(s->dh_top); cudaFree(s->dq); cudaFree(s->dv_part);
+  cudaFree(s->d_enc_out); cudaFree(s->d_enc_ht); cudaFree(s->dx0);
+  cudaFree(s->wa_t); cudaFree(s->wh_t); cudaFree(s->d_segs); cudaFree(s->d_sumsq);
   cudaFree(s->table_enc); cudaFree(s->table_dec); cudaFree(s->dec_rows); cudaFree(s->wy_t);
   for (int side = 0; side < 2; ++side)
     for (int l = 0; l < kMaxLayers; ++l) { cudaFree(s->w_cell[side][l]); cudaFree(s->b_cell[side][l]); }
@@ -719,6 +1118,8 @@ int n2nmn_seq2seq_set_weight(n2nmn_seq2seq* s, const char* name, const float* sr
                           (cudaStream_t)stream));
   v.loaded = true;
   s->dirty = true;
+  s->bwd_dirty = true;
+  s->rec_valid = false;
   return N2NMN_OK;
 }
 
@@ -748,6 +1149,12 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     return fail_with(N2NMN_ERR_CAPACITY, "T_enc / N exceed what the seq2seq was created for");
   if (!s->tables_set) return fail_with(N2NMN_ERR_STATE, "assembler tables (P, W, b) not set");
   auto st = (cudaStream_t)stream;
+  s->rec_valid = false;
+  const bool rec = s->record;
+  if (rec) {
+    const int rc = ensure_record(s);
+    if (rc) return rc;
+  }
   if (s->dirty) {
     const int rc = prepare(s, st);
     if (rc) return rc;
@@ -783,12 +1190,26 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     p.out_seq = l == NL - 1 ? out_seq : nullptr;
     p.seq_len = seq_len;
     p.t = t; p.N = N; p.L = L;
+    p.rec_gates = rec ? rec_gates_at(s, side, l, t, N) : nullptr;
+    p.rec_c = rec ? rec_state_at(s, s->rec_c[side], side, l, t, N) : nullptr;
+    p.rec_h = rec ? rec_state_at(s, s->rec_h[side], side, l, t, N) : nullptr;
     return p;
   };
   auto launch_wave = [&](const LstmWave& w, int nz, bool shared_sm) {
     const dim3 g3(grid.x, grid.y, nz), blk(kMmaThreads);
     cudaError_t le;
-    if (!narrow) {
+    if (rec) {
+      if (!narrow) {
+        le = exact ? launch(lstm_step_kernel<4, true, 3, true>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w)
+                   : launch(lstm_step_kernel<4, false, 3, true>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w);
+      } else if (shared_sm) {
+        le = exact ? launch(lstm_step_kernel<2, true, 3, true>, g3, blk, mma_smem_bytes(2, 3), st, kPdl, w)
+                   : launch(lstm_step_kernel<2, false, 3, true>, g3, blk, mma_smem_bytes(2, 3), st, kPdl, w);
+      } else {
+        le = exact ? launch(lstm_step_kernel<2, true, 5, true>, g3, blk, mma_smem_bytes(2, 5), st, kPdl, w)
+                   : launch(lstm_step_kernel<2, false, 5, true>, g3, blk, mma_smem_bytes(2, 5), st, kPdl, w);
+      }
+    } else if (!narrow) {
       le = exact ? launch(lstm_step_kernel<4, true, 3>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w)
                  : launch(lstm_step_kernel<4, false, 3>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w);
     } else if (shared_sm) {
@@ -832,11 +1253,12 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
   for (int t = 0; t < T_dec; ++t) {   // raw_rnn loop (:199-305)
     step(t, s->cur_tok);
     const float* h_top = s->h[NL - 1][cur];
+    float* q = rec ? s->rec_q + (size_t)t * N * L : s->q;   // the recording keeps every query
     rc = launch_gemm(s, st, h_top, L, N, L, s->v("decoder/att_prediction/weights"), L, L,
-                     s->v("decoder/att_prediction/biases"), s->q, L);
+                     s->v("decoder/att_prediction/biases"), q, L);
     if (rc) return rc;
     AttnStep a;
-    a.q = s->q; a.h_top = h_top; a.enc_ht = s->enc_ht; a.enc_out = s->enc_out;
+    a.q = q; a.h_top = h_top; a.enc_ht = s->enc_ht; a.enc_out = s->enc_out;
     a.v = s->v("decoder/att_prediction/v");
     a.wy_t = s->wy_t; a.by = s->v("decoder/token_prediction/biases");
     a.seq_len = seq_len_dev; a.P = s->P; a.W = s->W; a.b = s->b; a.X = s->X;
@@ -848,7 +1270,14 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     a.neg_entropy = neg_entropy_dev;
     a.atts = atts + (size_t)t * T_enc * N;
     a.T = T_enc; a.N = N; a.L = L; a.V = Vn;
-    if (launch(dec_attn_kernel, dim3(N), dim3(kAttnThreads), attn_smem, st, kPdl, a) != cudaSuccess)
+    a.rec_d2 = rec ? s->rec_d2 + (size_t)t * N * L : nullptr;
+    a.rec_sc = rec ? s->rec_sc + (size_t)t * N * Vn : nullptr;
+    a.rec_att = rec ? s->rec_att + (size_t)t * T_enc * N : nullptr;
+    a.rec_valid = rec ? s->rec_valid_bits + (size_t)t * N * 2 : nullptr;
+    a.rec_tok = rec ? s->rec_tok + (size_t)t * N : nullptr;
+    if ((rec ? launch(dec_attn_kernel<true>, dim3(N), dim3(kAttnThreads), attn_smem, st, kPdl, a)
+             : launch(dec_attn_kernel<false>, dim3(N), dim3(kAttnThreads), attn_smem, st, kPdl, a)) !=
+        cudaSuccess)
       ok = false;
     ++s->launches;
   }
@@ -857,6 +1286,14 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
   ++s->launches;
   S2S_TRY(cudaGetLastError());
   if (!ok) return fail_with(N2NMN_ERR_CUDA, "seq2seq kernel launch failed");
+  if (rec) {   // the inputs may be temporaries of the caller
+    S2S_TRY(cudaMemcpyAsync(s->rec_seq, input_seq_dev, sizeof(int32_t) * T_enc * N,
+                            cudaMemcpyDeviceToDevice, st));
+    S2S_TRY(cudaMemcpyAsync(s->rec_len, seq_len_dev, sizeof(int32_t) * N, cudaMemcpyDeviceToDevice, st));
+    s->rec_N = N;
+    s->rec_T = T_enc;
+    s->rec_valid = true;
+  }
   return N2NMN_OK;
 }
 
@@ -867,5 +1304,84 @@ int n2nmn_seq2seq_set_sampling(n2nmn_seq2seq* s, const float* uniforms_dev) {
 }
 
 int64_t n2nmn_seq2seq_launch_count(const n2nmn_seq2seq* s) { return s ? s->launches : 0; }
+
+int n2nmn_seq2seq_set_record(n2nmn_seq2seq* s, int on) {
+  if (!s) return fail_with(N2NMN_ERR_ARG, "null argument");
+  s->record = on != 0;
+  return N2NMN_OK;
+}
+
+int64_t n2nmn_seq2seq_flat_size(const n2nmn_seq2seq* s) { return s ? s->flat_size : 0; }
+
+int n2nmn_seq2seq_flat_offset(const n2nmn_seq2seq* s, int index, int64_t* offset, int64_t* count) {
+  if (!s || index < 0 || index >= (int)s->vars.size()) return fail_with(N2NMN_ERR_ARG, "bad variable index");
+  if (offset) *offset = s->vars[index].offset;
+  if (count) *count = (int64_t)s->vars[index].count;
+  return N2NMN_OK;
+}
+
+int n2nmn_seq2seq_backward(n2nmn_seq2seq* s, const float* d_log_seq_prob_dev,
+                           const float* d_neg_entropy_dev, const float* d_word_vecs_dev,
+                           float* grad_flat_dev, void* stream) {
+  if (!s || !grad_flat_dev) return fail_with(N2NMN_ERR_ARG, "null argument");
+  if (!s->rec_valid)
+    return fail_with(N2NMN_ERR_STATE,
+                     "seq2seq backward needs a recording forward of this batch (n2nmn_seq2seq_set_record) "
+                     "with no weight set since");
+  return backward_impl(s, d_log_seq_prob_dev, d_neg_entropy_dev, d_word_vecs_dev, grad_flat_dev,
+                       (cudaStream_t)stream);
+}
+
+int n2nmn_seq2seq_load_flat_weights(n2nmn_seq2seq* s, const float* wflat_dev, void* stream) {
+  if (!s || !wflat_dev) return fail_with(N2NMN_ERR_ARG, "null argument");
+  S2S_TRY(cudaMemcpyAsync(s->wstore, wflat_dev, sizeof(float) * s->flat_size,
+                          cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  for (auto& v : s->vars) v.loaded = true;
+  s->dirty = true;
+  s->bwd_dirty = true;
+  s->rec_valid = false;
+  return N2NMN_OK;
+}
+
+int n2nmn_seq2seq_get_flat_weights(const n2nmn_seq2seq* s, float* wflat_dev, void* stream) {
+  if (!s || !wflat_dev) return fail_with(N2NMN_ERR_ARG, "null argument");
+  S2S_TRY(cudaMemcpyAsync(wflat_dev, s->wstore, sizeof(float) * s->flat_size,
+                          cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return N2NMN_OK;
+}
+
+int n2nmn_seq2seq_adam_step(n2nmn_seq2seq* s, float* wflat_dev, float* gflat_dev, float* m_dev,
+                            float* v_dev, int step, float lr, float beta1, float beta2, float eps,
+                            float max_norm, float weight_decay, void* stream) {
+  if (!s || !wflat_dev || !gflat_dev || !m_dev || !v_dev || step < 1)
+    return fail_with(N2NMN_ERR_ARG, "bad argument");
+  auto st = (cudaStream_t)stream;
+  const int nv = (int)s->vars.size();
+  if (!s->segs_ready) {
+    std::vector<VarSeg> segs(nv);
+    for (int i = 0; i < nv; ++i) {
+      segs[i].offset = (int)s->vars[i].offset;
+      segs[i].count = (int)s->vars[i].count;
+      const std::string& n = s->vars[i].name;   // l2_reg covers ".../weights" only (nmn3_model.py:161-166)
+      segs[i].decay = n.size() >= 8 && n.compare(n.size() - 8, 8, "/weights") == 0;
+    }
+    S2S_TRY(dmalloc_once(&s->d_segs, (size_t)nv));
+    S2S_TRY(cudaMemcpy(s->d_segs, segs.data(), nv * sizeof(VarSeg), cudaMemcpyHostToDevice));
+    S2S_TRY(dmalloc_once(&s->d_sumsq, (size_t)nv));
+    s->segs_ready = true;
+  }
+  S2S_TRY(cudaMemsetAsync(s->d_sumsq, 0, nv * sizeof(float), st));
+  const dim3 grid(32, nv);
+  grad_norm_kernel<<<grid, 256, 0, st>>>(wflat_dev, gflat_dev, s->d_segs, weight_decay, 1.f,
+                                         s->d_sumsq, nullptr);
+  const double lr_t = (double)lr * std::sqrt(1.0 - std::pow((double)beta2, step)) /
+                      (1.0 - std::pow((double)beta1, step));
+  adam_clip_kernel<false><<<grid, 256, 0, st>>>(wflat_dev, gflat_dev, m_dev, v_dev, s->d_segs,
+                                                s->d_sumsq, (float)lr_t, beta1, beta2, eps, max_norm,
+                                                nullptr, nullptr, 0);
+  s->launches += 2;
+  S2S_TRY(cudaGetLastError());
+  return n2nmn_seq2seq_load_flat_weights(s, wflat_dev, stream);
+}
 
 }  // extern "C"

@@ -12,6 +12,10 @@ attribute names after a forward are the reference's: ``predicted_tokens`` [T_dec
 ``atts`` [T_decoder, T_encoder, N, 1]; ``log_seq_prob`` as nmn3_model.py:45 computes it.
 PyTorch only owns the device buffers; there is no CPU path.
 
+Training: ``forward(..., record=True)`` keeps what ``backward(d_log_seq_prob, d_neg_entropy,
+d_word_vecs)`` needs; the gradient of every variable lands in one flat buffer (``grads()`` gives
+``{TF name: view}``), the layout the optimiser step of ``trainer.LayoutGeneratorTrainer`` reads.
+
 `precision='fp32'` (default): every matrix product with fp32 parity (error-compensated TF32 on the
 tensor cores); `'tf32'`: one TF32 pass (13 % faster at batch 64, where the step is latency bound),
 probabilities within ~1e-3, a token may
@@ -122,13 +126,15 @@ class AttentionSeq2Seq:
                 check(self._L.n2nmn_seq2seq_set_weight(self._h, name.encode(), C.c_void_p(t.data_ptr()),
                                                        shp, len(shape), self._stream()))
                 torch.cuda.current_stream(self.device).synchronize()   # t may be a temporary
+        self._recorded_N = None
 
     def forward(self, input_seq_batch, seq_length_batch, use_gt_layout=None, gt_layout_batch=None,
-                sample_uniforms=None):
+                sample_uniforms=None, record=False):
         """input_seq_batch [T_enc, N] int, seq_length_batch [N] int (device or host);
         gt_layout_batch [T_decoder, N] with use_gt_layout truthy = teacher forcing;
         sample_uniforms [T_decoder, N] in [0, 1): the numbers the sampled decoding consumes
-        (decoder_sampling=True; default `torch.rand` on the device, i.e. torch's generator)."""
+        (decoder_sampling=True; default `torch.rand` on the device, i.e. torch's generator);
+        record=True keeps what `backward` needs (same outputs, bit for bit)."""
         dev = self.device
 
         def i32(x):
@@ -161,6 +167,7 @@ class AttentionSeq2Seq:
         wv = torch.empty((self.T_decoder, N, self.encoder_embed_dim), dtype=torch.float32, device=dev)
         atts = torch.empty((self.T_decoder, T, N, 1), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
+            check(self._L.n2nmn_seq2seq_set_record(self._h, 1 if record else 0))
             check(self._L.n2nmn_seq2seq_set_sampling(
                 self._h, C.c_void_p(u.data_ptr()) if u is not None else None))
             check(self._L.n2nmn_seq2seq_forward(
@@ -170,6 +177,7 @@ class AttentionSeq2Seq:
                 C.c_void_p(ent.data_ptr()), C.c_void_p(wv.data_ptr()), C.c_void_p(atts.data_ptr()),
                 self._stream()))
         self._keep = (seq, lens, gt, u)   # alive until the stream has consumed them
+        self._recorded_N = N if record else None
         self.predicted_tokens, self.token_probs, self.neg_entropy = tokens, probs, ent
         self.word_vecs, self.atts = wv, atts
         self.log_seq_prob = torch.log(probs).sum(0)          # nmn3_model.py:45
@@ -179,3 +187,71 @@ class AttentionSeq2Seq:
 
     def launch_count(self):
         return int(self._L.n2nmn_seq2seq_launch_count(self._h))
+
+    # ---- training -------------------------------------------------------------------------------
+    def flat_layout(self):
+        """(flat size, [(name, shape, offset, count)]) of the flat weight / gradient buffers."""
+        out = []
+        for i, (name, shape) in enumerate(self.variables()):
+            off, cnt = C.c_int64(), C.c_int64()
+            check(self._L.n2nmn_seq2seq_flat_offset(self._h, i, C.byref(off), C.byref(cnt)))
+            out.append((name, shape, off.value, cnt.value))
+        return int(self._L.n2nmn_seq2seq_flat_size(self._h)), out
+
+    def _views(self, flat):
+        return {name: flat[off:off + cnt].view(shape) for name, shape, off, cnt in self.flat_layout()[1]}
+
+    def get_flat_weights(self, out=None):
+        size = self.flat_layout()[0]
+        if out is None:
+            out = torch.zeros(size, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            check(self._L.n2nmn_seq2seq_get_flat_weights(self._h, C.c_void_p(out.data_ptr()),
+                                                         self._stream()))
+        return out
+
+    def load_flat_weights(self, wflat):
+        with torch.cuda.device(self.device):
+            check(self._L.n2nmn_seq2seq_load_flat_weights(self._h, C.c_void_p(wflat.data_ptr()),
+                                                          self._stream()))
+
+    def get_weights(self):
+        """{name relative to `<scope>/`: tensor}: the current variables, as `set_weights` takes them."""
+        return {k: v.clone() for k, v in self._views(self.get_flat_weights()).items()}
+
+    def backward(self, d_log_seq_prob=None, d_neg_entropy=None, d_word_vecs=None, out=None):
+        """Gradient of Σ d_log_seq_prob·log_seq_prob + Σ d_neg_entropy·neg_entropy +
+        Σ d_word_vecs·word_vecs with respect to every variable, after a `forward(..., record=True)`
+        of this batch (TF 1.0's gradients of nmn3_netgen_att.py; no gradient through the validity
+        masks or the chosen tokens). Upstreams: [N], [N], [T_decoder, N, embed_dim_txt] device
+        tensors or None (= zero). Returns the flat gradient buffer (`out`, or a new one); `grads()`
+        gives it per variable."""
+        N = getattr(self, '_recorded_N', None)
+        if N is None:
+            raise _lib.N2NMNError('backward needs a forward(..., record=True) of this batch')
+        dev = self.device
+
+        def f32(x, shape, what):
+            if x is None:
+                return None
+            t = (x if isinstance(x, torch.Tensor) else torch.as_tensor(np.asarray(x, np.float32)))
+            t = t.to(dev, torch.float32).contiguous()
+            if tuple(t.shape) != shape:
+                raise ValueError('%s must be %s (the recorded batch), got %s' % (what, shape, tuple(t.shape)))
+            return t
+        dlp = f32(d_log_seq_prob, (N,), 'd_log_seq_prob')
+        dne = f32(d_neg_entropy, (N,), 'd_neg_entropy')
+        dwv = f32(d_word_vecs, (self.T_decoder, N, self.encoder_embed_dim), 'd_word_vecs')
+        if out is None:
+            out = torch.empty(self.flat_layout()[0], dtype=torch.float32, device=dev)
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+        with torch.cuda.device(dev):
+            check(self._L.n2nmn_seq2seq_backward(self._h, ptr(dlp), ptr(dne), ptr(dwv), ptr(out),
+                                                 self._stream()))
+        self._bwd_keep = (dlp, dne, dwv)
+        self._grad = out
+        return out
+
+    def grads(self):
+        """{name relative to `<scope>/`: view of the last backward's gradient}."""
+        return self._views(self._grad)

@@ -196,3 +196,51 @@ class ModuleNetTrainer:
             out['total_loss'] = (pg + avg + self.lambda_entropy * entropy_reg +
                                  hp['weight_decay'] * l2)
         return out
+
+
+class LayoutGeneratorTrainer:
+    """Clip + Adam for the layout generator's variables (`seq2seq.AttentionSeq2Seq`), the
+    counterpart of `ModuleNetTrainer` for the other half of the reference's graph. It holds the
+    flat weights `w`, the gradient `g` and the Adam moments; `step()` runs the generator's backward
+    pass on its last recording forward and one optimiser step, all on the device.
+
+    The reference's two losses map onto the upstream gradients as follows (N = batch size):
+      gt-layout (exp_clevr/train_clevr_gt_layout.py:104-124): seq_likelihood_loss =
+        mean(-log_seq_prob) -> d_log_seq_prob = -1/N, plus d_word_vecs from
+        `ModuleNetTrainer.train_step(...)['d_word_vecs']`;
+      policy search (exp_clevr/train_clevr_rl_gt_layout.py:108-139): d_log_seq_prob =
+        `train_step(...)['reinforce_coeff']`, d_neg_entropy = lambda_entropy / N, plus
+        d_word_vecs.
+    weight_decay applies to every `.../weights` variable (the reference's l2_reg,
+    nmn3_model.py:161-166), not to the embeddings, go_embedding, v or the biases."""
+
+    def __init__(self, generator, lr=1e-4, beta1=0.9, beta2=0.999, eps=1e-8, max_grad_l2_norm=10.0,
+                 weight_decay=5e-6):
+        self.gen = generator
+        self._lib = _lib.lib()
+        dev = generator.device
+        self.flat_size = generator.flat_layout()[0]
+        self.w = generator.get_flat_weights()
+        self.g = torch.zeros(self.flat_size, dtype=torch.float32, device=dev)
+        self.m1 = torch.zeros(self.flat_size, dtype=torch.float32, device=dev)
+        self.m2 = torch.zeros(self.flat_size, dtype=torch.float32, device=dev)
+        self.step_count = 0
+        self.hyper = dict(lr=lr, beta1=beta1, beta2=beta2, eps=eps, max_norm=max_grad_l2_norm,
+                          weight_decay=weight_decay)
+
+    def grads(self):
+        return self.gen._views(self.g)
+
+    def step(self, d_log_seq_prob=None, d_neg_entropy=None, d_word_vecs=None):
+        """Backward pass of the generator's last `forward(..., record=True)`, then clip + Adam; the
+        generator takes the new weights (its next forward re-derives its packed copies)."""
+        self.gen.backward(d_log_seq_prob, d_neg_entropy, d_word_vecs, out=self.g)
+        self.step_count += 1
+        hp = self.hyper
+        dev = self.gen.device
+        with torch.cuda.device(dev):
+            _lib.check(self._lib.n2nmn_seq2seq_adam_step(
+                self.gen._h, self.w.data_ptr(), self.g.data_ptr(), self.m1.data_ptr(),
+                self.m2.data_ptr(), self.step_count, hp['lr'], hp['beta1'], hp['beta2'], hp['eps'],
+                hp['max_norm'], hp['weight_decay'], torch.cuda.current_stream(dev).cuda_stream))
+        self.gen._recorded_N = None

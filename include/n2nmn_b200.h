@@ -395,7 +395,7 @@ typedef struct n2nmn_seq2seq_config {
   int32_t embed_dim_txt;
   int32_t num_vocab_nmn;   /* <= 64 */
   int32_t embed_dim_nmn;
-  int32_t lstm_dim;        /* multiple of 16 */
+  int32_t lstm_dim;        /* multiple of 8 */
   int32_t num_layers;      /* <= 4 */
   int32_t T_encoder;       /* capacity, <= 128 */
   int32_t T_decoder;       /* decoding steps (fixed, as in the reference) */
@@ -439,6 +439,17 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
                           const int32_t* gt_layout_dev, int32_t* tokens_dev,
                           float* token_probs_dev, float* neg_entropy_dev, float* word_vecs_dev,
                           float* atts_dev, void* stream);
+/* n2nmn_seq2seq_forward plus the encoder's final state (models_vqa/nmn3_model.py passes it to the
+ * question-prior net): encoder_states_dev [num_layers][2][N][lstm_dim] receives (c, h) of every
+ * layer, LSTMStateTuple order, i.e. dynamic_rnn's final state — each question's state at its own
+ * length, carried to T_enc - 1 (nmn3_netgen_att.py:95-99), the state the decoder starts from.
+ * NULL = n2nmn_seq2seq_forward exactly. Copies only: the kernel launches are the same either way,
+ * (T_enc + num_layers - 1) + num_layers·T_decoder + 2·T_decoder + 3 per call. */
+int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
+                             const int32_t* seq_len_dev, int T_enc, int N,
+                             const int32_t* gt_layout_dev, int32_t* tokens_dev,
+                             float* token_probs_dev, float* neg_entropy_dev, float* word_vecs_dev,
+                             float* atts_dev, void* stream, float* encoder_states_dev);
 /* `decoder_sampling=True` (nmn3_netgen_att.py:234-256) for the following forward calls:
  * uniforms_dev [T_decoder][N] fp32 in [0,1) (N = the forward call's N; must stay valid until the
  * forward's work has run), one number per decoding step and question. The token is drawn from
@@ -469,6 +480,15 @@ int n2nmn_seq2seq_flat_offset(const n2nmn_seq2seq* s, int index, int64_t* offset
 int n2nmn_seq2seq_backward(n2nmn_seq2seq* s, const float* d_log_seq_prob_dev,
                            const float* d_neg_entropy_dev, const float* d_word_vecs_dev,
                            float* grad_flat_dev, void* stream);
+/* n2nmn_seq2seq_backward plus a fourth upstream gradient, d_encoder_states_dev
+ * [num_layers][2][N][lstm_dim] (dc, dh): d total / d encoder_states of n2nmn_seq2seq_forward_ex
+ * (e.g. from the question-prior net). It is added to the gradient of the encoder's final state that
+ * the decoder passes back and flows on through the carried rows in the same way. NULL = zero,
+ * i.e. n2nmn_seq2seq_backward exactly; otherwise one more launch. Same N2NMN_ERR_STATE rules. */
+int n2nmn_seq2seq_backward_ex(n2nmn_seq2seq* s, const float* d_log_seq_prob_dev,
+                              const float* d_neg_entropy_dev, const float* d_word_vecs_dev,
+                              float* grad_flat_dev, void* stream,
+                              const float* d_encoder_states_dev);
 /* All variables from / to one flat buffer (device, n2nmn_seq2seq_flat_offset layout). Loading
  * marks the derived weights for re-preparation at the next forward. */
 int n2nmn_seq2seq_load_flat_weights(n2nmn_seq2seq* s, const float* wflat_dev, void* stream);

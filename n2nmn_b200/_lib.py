@@ -50,10 +50,13 @@ SIGNATURES = {
     'n2nmn_seq2seq_set_weight': (C.c_int, [_P, C.c_char_p, _P, C.POINTER(C.c_int64), C.c_int, _P]),
     'n2nmn_seq2seq_set_assembler': (C.c_int, [_P, _I32P, _I32P, _I32P, _P]),
     'n2nmn_seq2seq_forward': (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
+    'n2nmn_seq2seq_forward_ex': (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P,
+                                           _P]),
     'n2nmn_seq2seq_set_sampling': (C.c_int, [_P, _P]),
     'n2nmn_seq2seq_launch_count': (C.c_int64, [_P]),
     'n2nmn_seq2seq_set_record': (C.c_int, [_P, C.c_int]),
     'n2nmn_seq2seq_backward': (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    'n2nmn_seq2seq_backward_ex': (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
     'n2nmn_seq2seq_flat_size': (C.c_int64, [_P]),
     'n2nmn_seq2seq_flat_offset': (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     'n2nmn_seq2seq_load_flat_weights': (C.c_int, [_P, _P, _P]),

@@ -805,7 +805,7 @@ int launch_colsum(n2nmn_seq2seq* s, cudaStream_t st, const float* in, int R, int
 XtbSrc xtb_src() { XtbSrc x; std::memset(&x, 0, sizeof(x)); return x; }
 
 int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const float* dwv,
-                  float* gflat, cudaStream_t st) {
+                  const float* dstates, float* gflat, cudaStream_t st) {
   const auto& g = s->cfg;
   const int L = g.lstm_dim, L4 = 4 * L, NL = g.num_layers, Vn = g.num_vocab_nmn;
   const int Vp = (Vn + 3) & ~3, Et = g.embed_dim_txt, En = g.embed_dim_nmn, Td = g.T_decoder;
@@ -893,6 +893,14 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
       gw.s[0] = gemm_slot(1, l, t);
       if ((rc = launch_bwd_gemm(s, st, gw, 1))) return rc;
     }
+  // drec / dc now hold the gradient of the encoder's final state from the decoder; the caller's
+  // gradient of that state (the question-prior net's input) joins it
+  if (dstates != nullptr) {
+    s2s_add_state_grad_kernel<<<dim3((N * L + 255) / 256, NL), 256, 0, st>>>(dstates, dc, drec, NLs,
+                                                                            N, L);
+    ++s->launches;
+    S2S_TRY(cudaGetLastError());
+  }
   // ---- 3. encoder: d enc_out += d enc_ht · W_hᵀ, encoder_h_transform gradients
   const int Re = T * N;
   rc = one_gemm(s, st, bwd_gemm(gemm_ops(s->d_enc_ht, L, Re, L, s->wh_t, L, L), s->d_enc_out, L,
@@ -970,13 +978,14 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
   if (!cfg || !out) return fail_with(N2NMN_ERR_ARG, "null argument");
   if (cfg->abi_version != N2NMN_ABI_VERSION) return fail_with(N2NMN_ERR_ARG, "ABI version mismatch");
   const int L = cfg->lstm_dim;
+  // lstm_dim: a multiple of 8, the units of one step-kernel CTA (8 units x 4 gates = 32 columns)
   if (cfg->num_vocab_txt <= 0 || cfg->embed_dim_txt <= 0 || cfg->embed_dim_nmn <= 0 ||
       cfg->embed_dim_txt % 4 != 0 || cfg->embed_dim_nmn % 4 != 0 ||
-      cfg->num_vocab_nmn <= 0 || cfg->num_vocab_nmn > kMaxVocabNmn || L <= 0 || L % 16 != 0 ||
+      cfg->num_vocab_nmn <= 0 || cfg->num_vocab_nmn > kMaxVocabNmn || L <= 0 || L % 8 != 0 ||
       cfg->num_layers <= 0 || cfg->num_layers > kMaxLayers || cfg->T_encoder <= 0 ||
       cfg->T_encoder > kMaxTEnc || cfg->T_decoder <= 0 || cfg->max_batch <= 0)
     return fail_with(N2NMN_ERR_ARG,
-                     "bad seq2seq config (lstm_dim must be a multiple of 16, embed dims of 4, num_vocab_nmn <= 64, "
+                     "bad seq2seq config (lstm_dim must be a multiple of 8, embed dims of 4, num_vocab_nmn <= 64, "
                      "num_layers <= 4, T_encoder <= 128)");
   S2S_TRY(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
@@ -984,6 +993,8 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
   if (prop.major != 9)
     return fail_with(N2NMN_ERR_DEVICE, std::string("n2nmn_b200 needs an sm_90 GPU, found sm_") +
                                            std::to_string(prop.major) + std::to_string(prop.minor));
+  if (head_bwd_smem_floats(L, cfg->T_encoder) * sizeof(float) > prop.sharedMemPerBlockOptin)
+    return fail_with(N2NMN_ERR_ARG, "lstm_dim too large for the backward head kernel's shared memory");
   auto* s = new n2nmn_seq2seq;
   s->cfg = *cfg;
   s->num_sms = prop.multiProcessorCount;
@@ -1061,7 +1072,7 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
   S2S_TRY(cudaFuncSetAttribute(lstm_step_kernel<2, true, 3>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   S2S_TRY(cudaFuncSetAttribute(lstm_step_kernel<2, false, 3>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   const size_t attn_bytes = attn_smem_floats(L, cfg->T_encoder, Vn) * sizeof(float);
-  if (attn_bytes > 200 * 1024)
+  if (attn_bytes > 200 * 1024 || attn_bytes > prop.sharedMemPerBlockOptin)
     return fail_with(N2NMN_ERR_ARG, "num_vocab_nmn * lstm_dim too large for the decoder step kernel");
   S2S_TRY(cudaFuncSetAttribute(dec_attn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)attn_bytes));
@@ -1141,6 +1152,16 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
                           const int32_t* gt_layout_dev, int32_t* tokens_dev,
                           float* token_probs_dev, float* neg_entropy_dev, float* word_vecs_dev,
                           float* atts_dev, void* stream) {
+  return n2nmn_seq2seq_forward_ex(s, input_seq_dev, seq_len_dev, T_enc, N, gt_layout_dev, tokens_dev,
+                                  token_probs_dev, neg_entropy_dev, word_vecs_dev, atts_dev, stream,
+                                  nullptr);
+}
+
+int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
+                             const int32_t* seq_len_dev, int T_enc, int N,
+                             const int32_t* gt_layout_dev, int32_t* tokens_dev,
+                             float* token_probs_dev, float* neg_entropy_dev, float* word_vecs_dev,
+                             float* atts_dev, void* stream, float* encoder_states_dev) {
   if (!s || !input_seq_dev || !seq_len_dev || !tokens_dev || !token_probs_dev ||
       !neg_entropy_dev || !word_vecs_dev)
     return fail_with(N2NMN_ERR_ARG, "null argument");
@@ -1235,6 +1256,15 @@ int n2nmn_seq2seq_forward(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     launch_wave(w, NL, NL > 1);
   }
   cur = T_enc & 1;
+  // dynamic_rnn's final state (:95-99), (c, h) per layer: the decoder's initial state, which its
+  // first step overwrites in place
+  if (encoder_states_dev != nullptr)
+    for (int l = 0; l < NL; ++l) {
+      float* dst = encoder_states_dev + (size_t)l * 2 * N * L;
+      S2S_TRY(cudaMemcpyAsync(dst, s->c[l], sizeof(float) * N * L, cudaMemcpyDeviceToDevice, st));
+      S2S_TRY(cudaMemcpyAsync(dst + (size_t)N * L, s->h[l][cur], sizeof(float) * N * L,
+                              cudaMemcpyDeviceToDevice, st));
+    }
   // decoder step: the layers of one step depend on each other, one launch each
   auto step = [&](int t, const int32_t* tok) {
     for (int l = 0; l < NL; ++l) {
@@ -1323,13 +1353,21 @@ int n2nmn_seq2seq_flat_offset(const n2nmn_seq2seq* s, int index, int64_t* offset
 int n2nmn_seq2seq_backward(n2nmn_seq2seq* s, const float* d_log_seq_prob_dev,
                            const float* d_neg_entropy_dev, const float* d_word_vecs_dev,
                            float* grad_flat_dev, void* stream) {
+  return n2nmn_seq2seq_backward_ex(s, d_log_seq_prob_dev, d_neg_entropy_dev, d_word_vecs_dev,
+                                   grad_flat_dev, stream, nullptr);
+}
+
+int n2nmn_seq2seq_backward_ex(n2nmn_seq2seq* s, const float* d_log_seq_prob_dev,
+                              const float* d_neg_entropy_dev, const float* d_word_vecs_dev,
+                              float* grad_flat_dev, void* stream,
+                              const float* d_encoder_states_dev) {
   if (!s || !grad_flat_dev) return fail_with(N2NMN_ERR_ARG, "null argument");
   if (!s->rec_valid)
     return fail_with(N2NMN_ERR_STATE,
                      "seq2seq backward needs a recording forward of this batch (n2nmn_seq2seq_set_record) "
                      "with no weight set since");
-  return backward_impl(s, d_log_seq_prob_dev, d_neg_entropy_dev, d_word_vecs_dev, grad_flat_dev,
-                       (cudaStream_t)stream);
+  return backward_impl(s, d_log_seq_prob_dev, d_neg_entropy_dev, d_word_vecs_dev,
+                       d_encoder_states_dev, grad_flat_dev, (cudaStream_t)stream);
 }
 
 int n2nmn_seq2seq_load_flat_weights(n2nmn_seq2seq* s, const float* wflat_dev, void* stream) {

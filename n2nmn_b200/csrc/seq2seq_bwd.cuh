@@ -9,6 +9,7 @@
 //                         dgates·W_xᵀ) on the mma_tile engine, one product per z slot
 //   s2s_xtb_kernel      : weight gradients out += Σ_r [x_r, h_r]ᵀ·g_r over all T·N rows (fp32)
 //   s2s_colsum_kernel   : bias gradients (column sums); s2s_scatter_rows_kernel: embedding rows
+//   s2s_add_state_grad_kernel: the caller's gradient of the encoder's final state (backward_ex)
 #pragma once
 #include "mma_tile.cuh"
 
@@ -212,6 +213,19 @@ __global__ void __launch_bounds__(256) s2s_cell_bwd_kernel(const CellBwdWave w) 
   dg[3 * L] = dh * tc * go * (1.f - go);
   p.dc[i] = dcc * gf;
   if (p.hcarry) p.hcarry[i] = 0.f;
+}
+
+// dc[l] += d_states[l][0], dh[l] += d_states[l][1]: the caller's gradient of the encoder's final
+// (c, h) [layers][2][N][L] added to the decoder's; grid = (ceil(N·L / 256), layers)
+__global__ void __launch_bounds__(256) s2s_add_state_grad_kernel(const float* __restrict__ d_states,
+                                                                 float* __restrict__ dc,
+                                                                 float* __restrict__ dh,
+                                                                 size_t layer_stride, int N, int L) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, l = blockIdx.y;
+  if (i >= N * L) return;
+  const float* src = d_states + (size_t)l * 2 * N * L;
+  dc[l * layer_stride + i] += src[i];
+  dh[l * layer_stride + i] += src[(size_t)N * L + i];
 }
 
 // out = [accumulate ? out : 0] + A·B on the mma_tile engine, columns [0, split) to out0 and

@@ -17,11 +17,15 @@ import torch
 
 
 def evaluate_split(pool, batches, assembler, answer_word_list, tst_image_set, save_file=None,
-                   eval_output_file=None, layout_fn=None, word_vecs_fn=None, max_in_flight=8):
+                   eval_output_file=None, layout_fn=None, word_vecs_fn=None, max_in_flight=8,
+                   score_prior_fn=None):
     """pool: ExecutorPool (batches are queued `max_in_flight` at a time and evaluated with dynamic
     batching); batches: iterable of data_reader dicts (n2nmn_b200.data.DataReader.batches());
     word_vecs_fn(batch) -> [T,N,Dt] float32 tensor (the seq2seq's attended word vectors; the
-    caller supplies them). Returns the dict of counts and accuracies that is also written out."""
+    caller supplies them). score_prior_fn(batch) -> [N, num_choices] float32 logits (tensor or
+    array) added to the module scores before the argmax: VQA's `scores_nmn + scores_qpn`
+    (exp_vqa/eval_vqa.py, use_qpn=True); None = the module scores alone. Returns the dict of counts
+    and accuracies that is also written out."""
     layout_fn = layout_fn or (lambda b: b['gt_layout_batch'])
     answer_correct = layout_correct = layout_valid = num_questions = 0
     output_answers = []
@@ -31,8 +35,11 @@ def evaluate_split(pool, batches, assembler, answer_word_list, tst_image_set, sa
         nonlocal answer_correct, layout_valid, num_questions
         pool.end()
         torch.cuda.synchronize(pool.device)
-        for batch, tokens, scores, valid in pending:
-            predictions = np.argmax(scores.cpu().numpy(), axis=1)
+        for batch, tokens, scores, valid, prior in pending:
+            s = scores.cpu().numpy()
+            if prior is not None:
+                s = s + prior
+            predictions = np.argmax(s, axis=1)
             if 'answer_label_batch' in batch:
                 answer_correct += int(np.sum(predictions == batch['answer_label_batch']))
             layout_valid += int(np.sum(valid))
@@ -53,7 +60,15 @@ def evaluate_split(pool, batches, assembler, answer_word_list, tst_image_set, sa
         feat = feat.to(pool.device, non_blocking=True)
         wv = word_vecs_fn(batch).to(pool.device, non_blocking=True)
         scores, valid, _ = pool.submit(feat, wv, tokens)
-        pending.append((batch, tokens, scores, valid))
+        prior = None
+        if score_prior_fn is not None:
+            prior = score_prior_fn(batch)
+            prior = (prior.detach().cpu().numpy() if isinstance(prior, torch.Tensor)
+                     else np.asarray(prior)).astype(np.float32)
+            if prior.shape != tuple(scores.shape):
+                raise ValueError('score_prior_fn must return [N, num_choices] = %r, got %r'
+                                 % (tuple(scores.shape), prior.shape))
+        pending.append((batch, tokens, scores, valid, prior))
         if len(pending) >= max_in_flight:
             flush()
     flush()

@@ -16,6 +16,11 @@ Training: ``forward(..., record=True)`` keeps what ``backward(d_log_seq_prob, d_
 d_word_vecs)`` needs; the gradient of every variable lands in one flat buffer (``grads()`` gives
 ``{TF name: view}``), the layout the optimiser step of ``trainer.LayoutGeneratorTrainer`` reads.
 
+VQA's question-prior net (models_vqa/question_prior_net.py) reads the encoder's final state:
+``forward(..., with_encoder_states=True)`` sets ``encoder_states``, a tuple of per-layer ``(c, h)``
+[N, lstm_dim] device views (TF's LSTMStateTuple order), and ``backward(..., d_encoder_states=)``
+takes the gradient of that state back.
+
 `precision='fp32'` (default): every matrix product with fp32 parity (error-compensated TF32 on the
 tensor cores); `'tf32'`: one TF32 pass (13 % faster at batch 64, where the step is latency bound),
 probabilities within ~1e-3, a token may
@@ -129,12 +134,15 @@ class AttentionSeq2Seq:
         self._recorded_N = None
 
     def forward(self, input_seq_batch, seq_length_batch, use_gt_layout=None, gt_layout_batch=None,
-                sample_uniforms=None, record=False):
+                sample_uniforms=None, record=False, with_encoder_states=False):
         """input_seq_batch [T_enc, N] int, seq_length_batch [N] int (device or host);
         gt_layout_batch [T_decoder, N] with use_gt_layout truthy = teacher forcing;
         sample_uniforms [T_decoder, N] in [0, 1): the numbers the sampled decoding consumes
         (decoder_sampling=True; default `torch.rand` on the device, i.e. torch's generator);
-        record=True keeps what `backward` needs (same outputs, bit for bit)."""
+        record=True keeps what `backward` needs (same outputs, bit for bit);
+        with_encoder_states=True also sets `self.encoder_states` = ((c, h) of layer 0, ...), each
+        [N, lstm_dim]: the encoder's final state (nmn3_netgen_att.py:95-99), which VQA's
+        question-prior net reads. Otherwise `self.encoder_states` is None."""
         dev = self.device
 
         def i32(x):
@@ -166,20 +174,26 @@ class AttentionSeq2Seq:
         ent = torch.empty((N,), dtype=torch.float32, device=dev)
         wv = torch.empty((self.T_decoder, N, self.encoder_embed_dim), dtype=torch.float32, device=dev)
         atts = torch.empty((self.T_decoder, T, N, 1), dtype=torch.float32, device=dev)
+        states = None
+        if with_encoder_states:
+            states = torch.empty((self.num_layers, 2, N, self.lstm_dim), dtype=torch.float32,
+                                 device=dev)
         with torch.cuda.device(dev):
             check(self._L.n2nmn_seq2seq_set_record(self._h, 1 if record else 0))
             check(self._L.n2nmn_seq2seq_set_sampling(
                 self._h, C.c_void_p(u.data_ptr()) if u is not None else None))
-            check(self._L.n2nmn_seq2seq_forward(
+            check(self._L.n2nmn_seq2seq_forward_ex(
                 self._h, C.c_void_p(seq.data_ptr()), C.c_void_p(lens.data_ptr()), T, N,
                 C.c_void_p(gt.data_ptr()) if gt is not None else None,
                 C.c_void_p(tokens.data_ptr()), C.c_void_p(probs.data_ptr()),
                 C.c_void_p(ent.data_ptr()), C.c_void_p(wv.data_ptr()), C.c_void_p(atts.data_ptr()),
-                self._stream()))
+                self._stream(), C.c_void_p(states.data_ptr()) if states is not None else None))
         self._keep = (seq, lens, gt, u)   # alive until the stream has consumed them
         self._recorded_N = N if record else None
         self.predicted_tokens, self.token_probs, self.neg_entropy = tokens, probs, ent
         self.word_vecs, self.atts = wv, atts
+        self.encoder_states = None if states is None else tuple(
+            (states[l, 0], states[l, 1]) for l in range(self.num_layers))
         self.log_seq_prob = torch.log(probs).sum(0)          # nmn3_model.py:45
         return tokens, probs, ent, wv, atts
 
@@ -219,13 +233,16 @@ class AttentionSeq2Seq:
         """{name relative to `<scope>/`: tensor}: the current variables, as `set_weights` takes them."""
         return {k: v.clone() for k, v in self._views(self.get_flat_weights()).items()}
 
-    def backward(self, d_log_seq_prob=None, d_neg_entropy=None, d_word_vecs=None, out=None):
+    def backward(self, d_log_seq_prob=None, d_neg_entropy=None, d_word_vecs=None, out=None,
+                 d_encoder_states=None):
         """Gradient of Σ d_log_seq_prob·log_seq_prob + Σ d_neg_entropy·neg_entropy +
-        Σ d_word_vecs·word_vecs with respect to every variable, after a `forward(..., record=True)`
-        of this batch (TF 1.0's gradients of nmn3_netgen_att.py; no gradient through the validity
-        masks or the chosen tokens). Upstreams: [N], [N], [T_decoder, N, embed_dim_txt] device
-        tensors or None (= zero). Returns the flat gradient buffer (`out`, or a new one); `grads()`
-        gives it per variable."""
+        Σ d_word_vecs·word_vecs + Σ d_encoder_states·encoder_states with respect to every variable,
+        after a `forward(..., record=True)` of this batch (TF 1.0's gradients of
+        nmn3_netgen_att.py; no gradient through the validity masks or the chosen tokens).
+        Upstreams: [N], [N], [T_decoder, N, embed_dim_txt] device tensors or None (= zero);
+        d_encoder_states in the shape of `encoder_states` (a tuple of per-layer (dc, dh) [N, L]) or
+        one [num_layers, 2, N, L] tensor, or None. Returns the flat gradient buffer (`out`, or a
+        new one); `grads()` gives it per variable."""
         N = getattr(self, '_recorded_N', None)
         if N is None:
             raise _lib.N2NMNError('backward needs a forward(..., record=True) of this batch')
@@ -242,13 +259,20 @@ class AttentionSeq2Seq:
         dlp = f32(d_log_seq_prob, (N,), 'd_log_seq_prob')
         dne = f32(d_neg_entropy, (N,), 'd_neg_entropy')
         dwv = f32(d_word_vecs, (self.T_decoder, N, self.encoder_embed_dim), 'd_word_vecs')
+        if isinstance(d_encoder_states, (tuple, list)):
+            if len(d_encoder_states) != self.num_layers:
+                raise ValueError('d_encoder_states must hold one (dc, dh) pair per layer')
+            d_encoder_states = torch.stack([torch.stack([f32(c, (N, self.lstm_dim), 'dc'),
+                                                         f32(h, (N, self.lstm_dim), 'dh')])
+                                            for c, h in d_encoder_states])
+        dst = f32(d_encoder_states, (self.num_layers, 2, N, self.lstm_dim), 'd_encoder_states')
         if out is None:
             out = torch.empty(self.flat_layout()[0], dtype=torch.float32, device=dev)
         ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
         with torch.cuda.device(dev):
-            check(self._L.n2nmn_seq2seq_backward(self._h, ptr(dlp), ptr(dne), ptr(dwv), ptr(out),
-                                                 self._stream()))
-        self._bwd_keep = (dlp, dne, dwv)
+            check(self._L.n2nmn_seq2seq_backward_ex(self._h, ptr(dlp), ptr(dne), ptr(dwv), ptr(out),
+                                                    self._stream(), ptr(dst)))
+        self._bwd_keep = (dlp, dne, dwv, dst)
         self._grad = out
         return out
 

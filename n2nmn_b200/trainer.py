@@ -212,7 +212,9 @@ class LayoutGeneratorTrainer:
         `train_step(...)['reinforce_coeff']`, d_neg_entropy = lambda_entropy / N, plus
         d_word_vecs.
     weight_decay applies to every `.../weights` variable (the reference's l2_reg,
-    nmn3_model.py:161-166), not to the embeddings, go_embedding, v or the biases."""
+    nmn3_model.py:161-166), not to the embeddings, go_embedding, v or the biases.
+    VQA (exp_vqa/train_vqa*.py, use_qpn=True) adds the question-prior net's input gradient:
+    d_encoder_states, the gradient of `generator.encoder_states` (see `AttentionSeq2Seq.backward`)."""
 
     def __init__(self, generator, lr=1e-4, beta1=0.9, beta2=0.999, eps=1e-8, max_grad_l2_norm=10.0,
                  weight_decay=5e-6):
@@ -231,10 +233,12 @@ class LayoutGeneratorTrainer:
     def grads(self):
         return self.gen._views(self.g)
 
-    def step(self, d_log_seq_prob=None, d_neg_entropy=None, d_word_vecs=None):
+    def step(self, d_log_seq_prob=None, d_neg_entropy=None, d_word_vecs=None,
+             d_encoder_states=None):
         """Backward pass of the generator's last `forward(..., record=True)`, then clip + Adam; the
         generator takes the new weights (its next forward re-derives its packed copies)."""
-        self.gen.backward(d_log_seq_prob, d_neg_entropy, d_word_vecs, out=self.g)
+        self.gen.backward(d_log_seq_prob, d_neg_entropy, d_word_vecs, out=self.g,
+                          d_encoder_states=d_encoder_states)
         self.step_count += 1
         hp = self.hyper
         dev = self.gen.device

@@ -40,18 +40,6 @@ int fail(int code, const std::string& msg) {
   return code;
 }
 
-#define CUDA_TRY(expr)                                                                  \
-  do {                                                                                  \
-    cudaError_t _e = (expr);                                                            \
-    if (_e != cudaSuccess)                                                              \
-      return fail(N2NMN_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));   \
-  } while (0)
-
-#define TRY(expr)                                                                       \
-  do {                                                                                  \
-    if (int _rc = (expr)) return _rc;                                                   \
-  } while (0)
-
 // Lazy workspaces allocate through this, so that a retry after a failed setup allocates only what
 // is still missing.
 template <class T>
@@ -361,19 +349,7 @@ void prof_mark(n2nmn_ctx* c, const char* name, cudaStream_t st) {
 template <class... KArgs, class... Args>
 int ctx_launch(n2nmn_ctx* c, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
                cudaStream_t st, LaunchAttrs a, Args... args) {
-  const cudaError_t e = launch(kernel, grid, block, smem, st, a, args...);
-  if (e != cudaSuccess) return fail(N2NMN_ERR_CUDA, std::string("kernel launch: ") + cudaGetErrorString(e));
-  ++c->launches;
-  return 0;
-}
-
-// Maximum dynamic shared memory of a kernel and, if carveout >= 0, its preferred carveout.
-template <class... KArgs>
-int set_smem(void (*kernel)(KArgs...), int bytes, int carveout = -1) {
-  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-  if (carveout >= 0)
-    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
-  return 0;
+  return launch(c->launches, kernel, grid, block, smem, st, a, args...);
 }
 
 // Kernel variants, chosen in one place for the attribute setup and the launch.

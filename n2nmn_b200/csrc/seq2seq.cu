@@ -34,6 +34,7 @@
 #include <cmath>
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -42,19 +43,9 @@
 #include "mma_tile.cuh"
 #include "optim.cuh"
 
-namespace n2nmn {
-int fail_with(int code, const std::string& msg);   // capi.cu: sets n2nmn_last_error()
-}
 using namespace n2nmn;
 
 namespace {
-
-#define S2S_TRY(expr)                                                                        \
-  do {                                                                                       \
-    cudaError_t _e = (expr);                                                                 \
-    if (_e != cudaSuccess)                                                                   \
-      return fail_with(N2NMN_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));  \
-  } while (0)
 
 constexpr int kMaxLayers = 4;
 constexpr int kAttnThreads = 512;
@@ -527,6 +518,7 @@ struct S2SVar {
 struct n2nmn_seq2seq {
   n2nmn_seq2seq_config cfg;
   int num_sms = 0;
+  std::vector<void*> allocs;   // every device buffer below (dmalloc), freed by destroy
   std::vector<S2SVar> vars;
   bool dirty = true, tables_set = false;
   const float* sample_u = nullptr;   // [T_decoder][N] uniforms of the following forward calls
@@ -573,31 +565,62 @@ struct n2nmn_seq2seq {
 
 namespace {
 
+// The kernels that call griddepcontrol.wait (s2s_gemm, lstm_step, dec_attn, s2s_bwd_gemm,
+// s2s_cell_bwd) launch with programmatic dependent launch; every other launch is plain.
 constexpr LaunchAttrs kPdl{true};
 
-// 32-row tiles while 64-row tiles would leave SMs without a CTA
-bool narrow_tiles(int col_blocks, int R, int num_sms) {
-  return R > 16 && col_blocks * ((R + 63) / 64) < num_sms;
+// Tile geometry of the mma_tile kernels for R rows, C columns and nz slots: 32-row tiles (WM = 2)
+// while 64-row tiles would leave SMs without a CTA.
+struct Tiles {
+  bool narrow;
+  dim3 grid;
+};
+Tiles tiles(int R, int C, int nz, int num_sms) {
+  const int cb = (C + kMmaCols - 1) / kMmaCols;
+  const bool narrow = R > 16 && cb * nz * ((R + 63) / 64) < num_sms;
+  return {narrow, dim3(cb, narrow ? (R + 31) / 32 : (R + 63) / 64, nz)};
+}
+
+// Kernel variants, chosen in one place for the attribute setup and the launch.
+auto gemm_variant(bool narrow, bool exact) {
+  if (narrow) return exact ? &s2s_gemm_kernel<2, true> : &s2s_gemm_kernel<2, false>;
+  return exact ? &s2s_gemm_kernel<4, true> : &s2s_gemm_kernel<4, false>;
+}
+auto bwd_gemm_variant(bool narrow, bool exact) {
+  if (narrow) return exact ? &s2s_bwd_gemm_kernel<2, true> : &s2s_bwd_gemm_kernel<2, false>;
+  return exact ? &s2s_bwd_gemm_kernel<4, true> : &s2s_bwd_gemm_kernel<4, false>;
+}
+// 64-row tiles run the 3-stage ring; 32-row tiles the 5-stage ring, or the 3-stage one where two
+// CTAs share an SM (the encoder wavefront)
+template <bool kRec>
+auto lstm_variant(bool narrow, bool shared_sm, bool exact) {
+  if (!narrow) return exact ? &lstm_step_kernel<4, true, 3, kRec> : &lstm_step_kernel<4, false, 3, kRec>;
+  if (shared_sm) return exact ? &lstm_step_kernel<2, true, 3, kRec> : &lstm_step_kernel<2, false, 3, kRec>;
+  return exact ? &lstm_step_kernel<2, true, 5, kRec> : &lstm_step_kernel<2, false, 5, kRec>;
+}
+auto lstm_variant(bool narrow, bool shared_sm, bool exact, bool rec) {
+  return rec ? lstm_variant<true>(narrow, shared_sm, exact)
+             : lstm_variant<false>(narrow, shared_sm, exact);
+}
+size_t lstm_smem(bool narrow, bool shared_sm) {
+  return mma_smem_bytes(narrow ? 2 : 4, narrow && !shared_sm ? 5 : 3);
+}
+
+GemmOperands gemm_ops(const float* A, int lda, int R, int K, const float* B, int ldb, int C) {
+  GemmOperands op;
+  op.a0 = A; op.k0 = K; op.lda0 = lda; op.a1 = nullptr; op.k1 = 0; op.lda1 = 0;
+  op.R = R; op.B = B; op.ldb = ldb; op.C = C;
+  return op;
 }
 
 int launch_gemm(n2nmn_seq2seq* s, cudaStream_t st, const float* A, int lda, int R, int K,
                 const float* B, int ldb, int C, const float* bias, float* out, int ldo,
                 bool force_exact = false) {
-  GemmOperands op;
-  op.a0 = A; op.k0 = K; op.lda0 = lda; op.a1 = nullptr; op.k1 = 0; op.lda1 = 0;
-  op.R = R; op.B = B; op.ldb = ldb; op.C = C;
-  const int cb = (C + kMmaCols - 1) / kMmaCols;
+  const Tiles t = tiles(R, C, 1, s->num_sms);
   const bool exact = !(s->cfg.flags & N2NMN_SEQ2SEQ_FLAG_TF32) || force_exact;
-  const dim3 gn(cb, (R + 31) / 32), gw(cb, (R + 63) / 64), blk(kMmaThreads);
-  if (narrow_tiles(cb, R, s->num_sms)) {
-    if (exact) S2S_TRY(launch(s2s_gemm_kernel<2, true>, gn, blk, mma_smem_bytes(2), st, kPdl, op, bias, out, ldo));
-    else S2S_TRY(launch(s2s_gemm_kernel<2, false>, gn, blk, mma_smem_bytes(2), st, kPdl, op, bias, out, ldo));
-  } else {
-    if (exact) S2S_TRY(launch(s2s_gemm_kernel<4, true>, gw, blk, mma_smem_bytes(4), st, kPdl, op, bias, out, ldo));
-    else S2S_TRY(launch(s2s_gemm_kernel<4, false>, gw, blk, mma_smem_bytes(4), st, kPdl, op, bias, out, ldo));
-  }
-  ++s->launches;
-  return N2NMN_OK;
+  return launch(s->launches, gemm_variant(t.narrow, exact), t.grid, kMmaThreads,
+                mma_smem_bytes(t.narrow ? 2 : 4), st, kPdl, gemm_ops(A, lda, R, K, B, ldb, C), bias,
+                out, ldo);
 }
 
 std::string cell_prefix(int side, int l) {
@@ -614,37 +637,40 @@ int prepare(n2nmn_seq2seq* s, cudaStream_t st) {
   for (int side = 0; side < 2; ++side) {
     for (int l = 0; l < g.num_layers; ++l) {
       const int in = l == 0 ? (side == 0 ? g.embed_dim_txt : g.embed_dim_nmn) : L;
-      regroup_gates_kernel<<<s->num_sms, 256, 0, st>>>(s->v(cell_prefix(side, l) + "weights"),
-                                                s->w_cell[side][l], in + L, L);
-      regroup_gates_kernel<<<8, 256, 0, st>>>(s->v(cell_prefix(side, l) + "biases"),
-                                              s->b_cell[side][l], 1, L);
-      s->launches += 2;
+      TRY(launch(s->launches, regroup_gates_kernel, s->num_sms, 256, 0, st, {},
+                 s->v(cell_prefix(side, l) + "weights"), s->w_cell[side][l], in + L, L));
+      TRY(launch(s->launches, regroup_gates_kernel, 8, 256, 0, st, {},
+                 s->v(cell_prefix(side, l) + "biases"), s->b_cell[side][l], 1, L));
     }
   }
-  S2S_TRY(cudaMemcpyAsync(s->dec_rows, s->v("decoder/embedding_mat"),
-                          sizeof(float) * g.num_vocab_nmn * g.embed_dim_nmn,
-                          cudaMemcpyDeviceToDevice, st));
-  S2S_TRY(cudaMemcpyAsync(s->dec_rows + (size_t)g.num_vocab_nmn * g.embed_dim_nmn,
-                          s->v("decoder/go_embedding"), sizeof(float) * g.embed_dim_nmn,
-                          cudaMemcpyDeviceToDevice, st));
-  int rc = launch_gemm(s, st, s->v("encoder/embedding_mat"), g.embed_dim_txt, g.num_vocab_txt,
-                       g.embed_dim_txt, s->w_cell[0][0], C, C, nullptr, s->table_enc, C, true);
-  if (rc) return rc;
-  rc = launch_gemm(s, st, s->dec_rows, g.embed_dim_nmn, g.num_vocab_nmn + 1, g.embed_dim_nmn,
-                   s->w_cell[1][0], C, C, nullptr, s->table_dec, C, true);
-  if (rc) return rc;
-  transpose_kernel<<<64, 256, 0, st>>>(s->v("decoder/token_prediction/weights"), s->wy_t, 2 * L,
-                                       g.num_vocab_nmn);
-  ++s->launches;
-  S2S_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(s->dec_rows, s->v("decoder/embedding_mat"),
+                           sizeof(float) * g.num_vocab_nmn * g.embed_dim_nmn,
+                           cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(s->dec_rows + (size_t)g.num_vocab_nmn * g.embed_dim_nmn,
+                           s->v("decoder/go_embedding"), sizeof(float) * g.embed_dim_nmn,
+                           cudaMemcpyDeviceToDevice, st));
+  TRY(launch_gemm(s, st, s->v("encoder/embedding_mat"), g.embed_dim_txt, g.num_vocab_txt,
+                  g.embed_dim_txt, s->w_cell[0][0], C, C, nullptr, s->table_enc, C, true));
+  TRY(launch_gemm(s, st, s->dec_rows, g.embed_dim_nmn, g.num_vocab_nmn + 1, g.embed_dim_nmn,
+                  s->w_cell[1][0], C, C, nullptr, s->table_dec, C, true));
+  TRY(launch(s->launches, transpose_kernel, 64, 256, 0, st, {},
+             s->v("decoder/token_prediction/weights"), s->wy_t, 2 * L, g.num_vocab_nmn));
   s->dirty = false;
   return N2NMN_OK;
 }
 
+// Every device buffer of the context is allocated here and recorded for n2nmn_seq2seq_destroy.
 template <class T>
-cudaError_t dmalloc(T** p, size_t n) { return cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)); }
+cudaError_t dmalloc(n2nmn_seq2seq* s, T** p, size_t n) {
+  const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T));
+  if (e == cudaSuccess) s->allocs.push_back(*p);
+  return e;
+}
+// Lazy workspaces: a retry after a failed attempt allocates only what is still missing.
 template <class T>
-cudaError_t dmalloc_once(T** p, size_t n) { return *p ? cudaSuccess : dmalloc(p, n); }
+cudaError_t dmalloc_once(n2nmn_seq2seq* s, T** p, size_t n) {
+  return *p ? cudaSuccess : dmalloc(s, p, n);
+}
 
 int t_cap(const n2nmn_seq2seq* s, int side) { return side == 0 ? s->cfg.T_encoder : s->cfg.T_decoder; }
 // recorded rows of (side, layer) from step t on, with the recorded batch size N
@@ -670,51 +696,34 @@ int ensure_record(n2nmn_seq2seq* s) {
   const size_t Te = g.T_encoder, Vn = g.num_vocab_nmn, Vp = (Vn + 3) & ~size_t(3);
   for (int side = 0; side < 2; ++side) {
     const size_t rows = NL * (size_t)t_cap(s, side) * N;
-    S2S_TRY(dmalloc_once(&s->rec_gates[side], rows * 4 * L));
-    S2S_TRY(dmalloc_once(&s->rec_c[side], rows * L));
-    S2S_TRY(dmalloc_once(&s->rec_h[side], rows * L));
-    S2S_TRY(dmalloc_once(&s->dgates[side], rows * 4 * L));
+    CUDA_TRY(dmalloc_once(s, &s->rec_gates[side], rows * 4 * L));
+    CUDA_TRY(dmalloc_once(s, &s->rec_c[side], rows * L));
+    CUDA_TRY(dmalloc_once(s, &s->rec_h[side], rows * L));
+    CUDA_TRY(dmalloc_once(s, &s->dgates[side], rows * 4 * L));
     for (size_t l = 0; l < NL; ++l) {
       const size_t in = l == 0 ? (side == 0 ? g.embed_dim_txt : g.embed_dim_nmn) : L;
-      S2S_TRY(dmalloc_once(&s->w_t[side][l], 4 * L * (in + L)));
+      CUDA_TRY(dmalloc_once(s, &s->w_t[side][l], 4 * L * (in + L)));
     }
   }
-  S2S_TRY(dmalloc_once(&s->rec_q, Td * N * L));
-  S2S_TRY(dmalloc_once(&s->rec_d2, Td * N * L));
-  S2S_TRY(dmalloc_once(&s->rec_sc, Td * N * Vn));
-  S2S_TRY(dmalloc_once(&s->rec_att, Td * Te * N));
-  S2S_TRY(dmalloc_once(&s->rec_valid_bits, Td * N * 2));
-  S2S_TRY(dmalloc_once(&s->rec_tok, Td * N));
-  S2S_TRY(dmalloc_once(&s->rec_seq, Te * N));
-  S2S_TRY(dmalloc_once(&s->rec_len, N));
-  for (auto*& p : s->d_h) S2S_TRY(dmalloc_once(&p, NL * N * L));
-  S2S_TRY(dmalloc_once(&s->ds, Td * N * Vp));
-  S2S_TRY(dmalloc_once(&s->dh_top, Td * N * L));
-  S2S_TRY(dmalloc_once(&s->dq, Td * N * L));
-  S2S_TRY(dmalloc_once(&s->dv_part, N * L));
-  S2S_TRY(dmalloc_once(&s->d_enc_out, Te * N * L));
-  S2S_TRY(dmalloc_once(&s->d_enc_ht, Te * N * L));
+  CUDA_TRY(dmalloc_once(s, &s->rec_q, Td * N * L));
+  CUDA_TRY(dmalloc_once(s, &s->rec_d2, Td * N * L));
+  CUDA_TRY(dmalloc_once(s, &s->rec_sc, Td * N * Vn));
+  CUDA_TRY(dmalloc_once(s, &s->rec_att, Td * Te * N));
+  CUDA_TRY(dmalloc_once(s, &s->rec_valid_bits, Td * N * 2));
+  CUDA_TRY(dmalloc_once(s, &s->rec_tok, Td * N));
+  CUDA_TRY(dmalloc_once(s, &s->rec_seq, Te * N));
+  CUDA_TRY(dmalloc_once(s, &s->rec_len, N));
+  for (auto*& p : s->d_h) CUDA_TRY(dmalloc_once(s, &p, NL * N * L));
+  CUDA_TRY(dmalloc_once(s, &s->ds, Td * N * Vp));
+  CUDA_TRY(dmalloc_once(s, &s->dh_top, Td * N * L));
+  CUDA_TRY(dmalloc_once(s, &s->dq, Td * N * L));
+  CUDA_TRY(dmalloc_once(s, &s->dv_part, N * L));
+  CUDA_TRY(dmalloc_once(s, &s->d_enc_out, Te * N * L));
+  CUDA_TRY(dmalloc_once(s, &s->d_enc_ht, Te * N * L));
   const size_t E = std::max(g.embed_dim_txt * Te, g.embed_dim_nmn * Td);
-  S2S_TRY(dmalloc_once(&s->dx0, E * N));
-  S2S_TRY(dmalloc_once(&s->wa_t, L * L));
-  S2S_TRY(dmalloc_once(&s->wh_t, L * L));
-  auto opt_in = [](auto kernel, size_t bytes) {
-    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  };
-  S2S_TRY(opt_in(lstm_step_kernel<2, true, 5, true>, mma_smem_bytes(2, 5)));
-  S2S_TRY(opt_in(lstm_step_kernel<2, false, 5, true>, mma_smem_bytes(2, 5)));
-  S2S_TRY(opt_in(lstm_step_kernel<2, true, 3, true>, mma_smem_bytes(2, 3)));
-  S2S_TRY(opt_in(lstm_step_kernel<2, false, 3, true>, mma_smem_bytes(2, 3)));
-  S2S_TRY(opt_in(lstm_step_kernel<4, true, 3, true>, mma_smem_bytes(4, 3)));
-  S2S_TRY(opt_in(lstm_step_kernel<4, false, 3, true>, mma_smem_bytes(4, 3)));
-  S2S_TRY(cudaFuncSetAttribute(lstm_step_kernel<2, true, 3, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  S2S_TRY(cudaFuncSetAttribute(lstm_step_kernel<2, false, 3, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  S2S_TRY(opt_in(dec_attn_kernel<true>, attn_smem_floats(g.lstm_dim, g.T_encoder, Vn) * sizeof(float)));
-  S2S_TRY(opt_in(s2s_bwd_gemm_kernel<2, true>, mma_smem_bytes(2)));
-  S2S_TRY(opt_in(s2s_bwd_gemm_kernel<2, false>, mma_smem_bytes(2)));
-  S2S_TRY(opt_in(s2s_bwd_gemm_kernel<4, true>, mma_smem_bytes(4)));
-  S2S_TRY(opt_in(s2s_bwd_gemm_kernel<4, false>, mma_smem_bytes(4)));
-  S2S_TRY(opt_in(s2s_head_bwd_kernel, head_bwd_smem_floats(g.lstm_dim, g.T_encoder) * sizeof(float)));
+  CUDA_TRY(dmalloc_once(s, &s->dx0, E * N));
+  CUDA_TRY(dmalloc_once(s, &s->wa_t, L * L));
+  CUDA_TRY(dmalloc_once(s, &s->wh_t, L * L));
   s->rec_ready = true;
   return N2NMN_OK;
 }
@@ -727,43 +736,25 @@ int prepare_backward(n2nmn_seq2seq* s, cudaStream_t st) {
   for (int side = 0; side < 2; ++side)
     for (int l = 0; l < g.num_layers; ++l) {
       const int in = l == 0 ? (side == 0 ? g.embed_dim_txt : g.embed_dim_nmn) : L;
-      transpose_kernel<<<s->num_sms, 256, 0, st>>>(s->v(cell_prefix(side, l) + "weights"),
-                                                   s->w_t[side][l], in + L, 4 * L);
-      ++s->launches;
+      TRY(launch(s->launches, transpose_kernel, s->num_sms, 256, 0, st, {},
+                 s->v(cell_prefix(side, l) + "weights"), s->w_t[side][l], in + L, 4 * L));
     }
-  transpose_kernel<<<64, 256, 0, st>>>(s->v("decoder/att_prediction/weights"), s->wa_t, L, L);
-  transpose_kernel<<<64, 256, 0, st>>>(s->v("encoder/encoder_h_transform/weights"), s->wh_t, L, L);
-  s->launches += 2;
-  S2S_TRY(cudaGetLastError());
+  TRY(launch(s->launches, transpose_kernel, 64, 256, 0, st, {},
+             s->v("decoder/att_prediction/weights"), s->wa_t, L, L));
+  TRY(launch(s->launches, transpose_kernel, 64, 256, 0, st, {},
+             s->v("encoder/encoder_h_transform/weights"), s->wh_t, L, L));
   s->bwd_dirty = false;
   return N2NMN_OK;
-}
-
-GemmOperands gemm_ops(const float* A, int lda, int R, int K, const float* B, int ldb, int C) {
-  GemmOperands op;
-  op.a0 = A; op.k0 = K; op.lda0 = lda; op.a1 = nullptr; op.k1 = 0; op.lda1 = 0;
-  op.R = R; op.B = B; op.ldb = ldb; op.C = C;
-  return op;
 }
 
 // One launch of s2s_bwd_gemm_kernel over `nz` slots; exact = the error-compensated 3xTF32 path.
 int launch_bwd_gemm(n2nmn_seq2seq* s, cudaStream_t st, const BwdGemmWave& w, int nz) {
   int R = 0, C = 0;
   for (int z = 0; z < nz; ++z) { R = std::max(R, w.s[z].op.R); C = std::max(C, w.s[z].op.C); }
-  const int cb = (C + kMmaCols - 1) / kMmaCols;
+  const Tiles t = tiles(R, C, nz, s->num_sms);
   const bool exact = !(s->cfg.flags & N2NMN_SEQ2SEQ_FLAG_TF32);
-  const dim3 blk(kMmaThreads);
-  if (narrow_tiles(cb * nz, R, s->num_sms)) {
-    const dim3 grid(cb, (R + 31) / 32, nz);
-    S2S_TRY(exact ? launch(s2s_bwd_gemm_kernel<2, true>, grid, blk, mma_smem_bytes(2), st, kPdl, w)
-                  : launch(s2s_bwd_gemm_kernel<2, false>, grid, blk, mma_smem_bytes(2), st, kPdl, w));
-  } else {
-    const dim3 grid(cb, (R + 63) / 64, nz);
-    S2S_TRY(exact ? launch(s2s_bwd_gemm_kernel<4, true>, grid, blk, mma_smem_bytes(4), st, kPdl, w)
-                  : launch(s2s_bwd_gemm_kernel<4, false>, grid, blk, mma_smem_bytes(4), st, kPdl, w));
-  }
-  ++s->launches;
-  return N2NMN_OK;
+  return launch(s->launches, bwd_gemm_variant(t.narrow, exact), t.grid, kMmaThreads,
+                mma_smem_bytes(t.narrow ? 2 : 4), st, kPdl, w);
 }
 
 BwdGemm bwd_gemm(GemmOperands op, float* out0, int ldo0, float* out1, int ldo1, int split,
@@ -787,19 +778,13 @@ int launch_xtb(n2nmn_seq2seq* s, cudaStream_t st, const XtbSrc& x) {
   const int tiles = grid0.x * grid0.y;
   // split the rows while the tiles alone leave SMs idle, keeping >= 128 rows per split
   int splits = std::max(1, std::min((2 * s->num_sms + tiles - 1) / tiles, x.R / 128));
-  s2s_xtb_kernel<<<dim3(grid0.x, grid0.y, splits), 256, 0, st>>>(x);
-  ++s->launches;
-  S2S_TRY(cudaGetLastError());
-  return N2NMN_OK;
+  return launch(s->launches, s2s_xtb_kernel, dim3(grid0.x, grid0.y, splits), 256, 0, st, {}, x);
 }
 
 int launch_colsum(n2nmn_seq2seq* s, cudaStream_t st, const float* in, int R, int ld, int C, float* out) {
   const int cb = (C + 255) / 256;
   const int splits = std::max(1, std::min((2 * s->num_sms + cb - 1) / cb, R / 64));
-  s2s_colsum_kernel<<<dim3(cb, splits), 256, 0, st>>>(in, R, ld, C, out);
-  ++s->launches;
-  S2S_TRY(cudaGetLastError());
-  return N2NMN_OK;
+  return launch(s->launches, s2s_colsum_kernel, dim3(cb, splits), 256, 0, st, {}, in, R, ld, C, out);
 }
 
 XtbSrc xtb_src() { XtbSrc x; std::memset(&x, 0, sizeof(x)); return x; }
@@ -811,14 +796,11 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
   const int Vp = (Vn + 3) & ~3, Et = g.embed_dim_txt, En = g.embed_dim_nmn, Td = g.T_decoder;
   const int N = s->rec_N, T = s->rec_T;
   auto off = [&](const std::string& name) { return gflat + s->vars[s->var(name)].offset; };
-  if (s->bwd_dirty) {
-    const int rc = prepare_backward(s, st);
-    if (rc) return rc;
-  }
-  S2S_TRY(cudaMemsetAsync(gflat, 0, sizeof(float) * s->flat_size, st));
-  for (auto* p : s->d_h) S2S_TRY(cudaMemsetAsync(p, 0, sizeof(float) * NL * g.max_batch * L, st));
-  S2S_TRY(cudaMemsetAsync(s->d_enc_out, 0, sizeof(float) * T * N * L, st));
-  S2S_TRY(cudaMemsetAsync(s->d_enc_ht, 0, sizeof(float) * T * N * L, st));
+  if (s->bwd_dirty) TRY(prepare_backward(s, st));
+  CUDA_TRY(cudaMemsetAsync(gflat, 0, sizeof(float) * s->flat_size, st));
+  for (auto* p : s->d_h) CUDA_TRY(cudaMemsetAsync(p, 0, sizeof(float) * NL * g.max_batch * L, st));
+  CUDA_TRY(cudaMemsetAsync(s->d_enc_out, 0, sizeof(float) * T * N * L, st));
+  CUDA_TRY(cudaMemsetAsync(s->d_enc_ht, 0, sizeof(float) * T * N * L, st));
   float *drec = s->d_h[0], *dup = s->d_h[1], *hcarry = s->d_h[2], *dc = s->d_h[3];
   const size_t NLs = (size_t)g.max_batch * L;   // per-layer stride of the dh buffers
   // ---- 1. decoder head, every step at once
@@ -831,27 +813,25 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
   hb.ds = s->ds; hb.dh_top = s->dh_top; hb.dq = s->dq; hb.d_enc_out = s->d_enc_out;
   hb.d_enc_ht = s->d_enc_ht; hb.dv_part = s->dv_part; hb.d_emb_txt = off("encoder/embedding_mat");
   hb.T = T; hb.N = N; hb.L = L; hb.V = Vn; hb.Vp = Vp; hb.Td = Td; hb.E = Et;
-  s2s_head_bwd_kernel<<<N, kHeadBwdThreads, head_bwd_smem_floats(L, T) * sizeof(float), st>>>(hb);
-  ++s->launches;
-  S2S_TRY(cudaGetLastError());
+  TRY(launch(s->launches, s2s_head_bwd_kernel, N, kHeadBwdThreads,
+             head_bwd_smem_floats(L, T) * sizeof(float), st, {}, hb));
   // dh_top += dq · W_aᵀ over all T_dec·N rows; att_prediction, token_prediction and v gradients
   const int Rd = Td * N;
   const float* h_top = rec_state_at(s, s->rec_h[1], 1, NL - 1, 0, N);   // [Td·N][L]
-  int rc = one_gemm(s, st, bwd_gemm(gemm_ops(s->dq, L, Rd, L, s->wa_t, L, L), s->dh_top, L,
-                                    nullptr, 0, L, true));
-  if (rc) return rc;
+  TRY(one_gemm(s, st, bwd_gemm(gemm_ops(s->dq, L, Rd, L, s->wa_t, L, L), s->dh_top, L, nullptr, 0,
+                               L, true)));
   XtbSrc x = xtb_src();
   x.x = h_top; x.ldx = L; x.kx = L; x.G = s->dq; x.ldg = L; x.C = L; x.R = Rd;
   x.out = off("decoder/att_prediction/weights"); x.ldo = L;
-  if ((rc = launch_xtb(s, st, x))) return rc;
-  if ((rc = launch_colsum(s, st, s->dq, Rd, L, L, off("decoder/att_prediction/biases")))) return rc;
+  TRY(launch_xtb(s, st, x));
+  TRY(launch_colsum(s, st, s->dq, Rd, L, L, off("decoder/att_prediction/biases")));
   x = xtb_src();
   x.x = h_top; x.ldx = L; x.kx = L; x.hb = s->rec_d2; x.ldh = L; x.kh = L;
   x.G = s->ds; x.ldg = Vp; x.C = Vn; x.R = Rd;
   x.out = off("decoder/token_prediction/weights"); x.ldo = Vn;
-  if ((rc = launch_xtb(s, st, x))) return rc;
-  if ((rc = launch_colsum(s, st, s->ds, Rd, Vp, Vn, off("decoder/token_prediction/biases")))) return rc;
-  if ((rc = launch_colsum(s, st, s->dv_part, N, L, L, off("decoder/att_prediction/v")))) return rc;
+  TRY(launch_xtb(s, st, x));
+  TRY(launch_colsum(s, st, s->ds, Rd, Vp, Vn, off("decoder/token_prediction/biases")));
+  TRY(launch_colsum(s, st, s->dv_part, N, L, L, off("decoder/att_prediction/v")));
   // ---- 2. decoder BPTT, one cell backward and one [dx, dh_prev] product per layer and step
   auto in_dim = [&](int side, int l) { return l == 0 ? (side == 0 ? Et : En) : L; };
   auto cell_slot = [&](int side, int l, int t) {
@@ -878,40 +858,34 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
                     false);
   };
   auto launch_cells = [&](const CellBwdWave& w, int nz) {
-    const dim3 grid((N * L + 255) / 256, 1, nz);
-    ++s->launches;
-    return launch(s2s_cell_bwd_kernel, grid, dim3(256), 0, st, kPdl, w);
+    return launch(s->launches, s2s_cell_bwd_kernel, dim3((N * L + 255) / 256, 1, nz), 256, 0, st,
+                  kPdl, w);
   };
   for (int t = Td - 1; t >= 0; --t)
     for (int l = NL - 1; l >= 0; --l) {
       CellBwdWave cw;
       std::memset(&cw, 0, sizeof(cw));
       cw.s[0] = cell_slot(1, l, t);
-      S2S_TRY(launch_cells(cw, 1));
+      TRY(launch_cells(cw, 1));
       BwdGemmWave gw;
       std::memset(&gw, 0, sizeof(gw));
       gw.s[0] = gemm_slot(1, l, t);
-      if ((rc = launch_bwd_gemm(s, st, gw, 1))) return rc;
+      TRY(launch_bwd_gemm(s, st, gw, 1));
     }
   // drec / dc now hold the gradient of the encoder's final state from the decoder; the caller's
   // gradient of that state (the question-prior net's input) joins it
-  if (dstates != nullptr) {
-    s2s_add_state_grad_kernel<<<dim3((N * L + 255) / 256, NL), 256, 0, st>>>(dstates, dc, drec, NLs,
-                                                                            N, L);
-    ++s->launches;
-    S2S_TRY(cudaGetLastError());
-  }
+  if (dstates != nullptr)
+    TRY(launch(s->launches, s2s_add_state_grad_kernel, dim3((N * L + 255) / 256, NL), 256, 0, st, {},
+               dstates, dc, drec, NLs, N, L));
   // ---- 3. encoder: d enc_out += d enc_ht · W_hᵀ, encoder_h_transform gradients
   const int Re = T * N;
-  rc = one_gemm(s, st, bwd_gemm(gemm_ops(s->d_enc_ht, L, Re, L, s->wh_t, L, L), s->d_enc_out, L,
-                                nullptr, 0, L, true));
-  if (rc) return rc;
+  TRY(one_gemm(s, st, bwd_gemm(gemm_ops(s->d_enc_ht, L, Re, L, s->wh_t, L, L), s->d_enc_out, L,
+                               nullptr, 0, L, true)));
   x = xtb_src();
   x.x = s->enc_out; x.ldx = L; x.kx = L; x.G = s->d_enc_ht; x.ldg = L; x.C = L; x.R = Re;
   x.out = off("encoder/encoder_h_transform/weights"); x.ldo = L;
-  if ((rc = launch_xtb(s, st, x))) return rc;
-  if ((rc = launch_colsum(s, st, s->d_enc_ht, Re, L, L, off("encoder/encoder_h_transform/biases"))))
-    return rc;
+  TRY(launch_xtb(s, st, x));
+  TRY(launch_colsum(s, st, s->d_enc_ht, Re, L, L, off("encoder/encoder_h_transform/biases")));
   // reverse wavefront: tick k runs layer l at step t = T - 1 - k + (layers - 1 - l)
   for (int k = 0; k < T + NL - 1; ++k) {
     CellBwdWave cw;
@@ -924,8 +898,8 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
       cw.s[l] = cell_slot(0, l, t);
       gw.s[l] = gemm_slot(0, l, t);
     }
-    S2S_TRY(launch_cells(cw, NL));
-    if ((rc = launch_bwd_gemm(s, st, gw, NL))) return rc;
+    TRY(launch_cells(cw, NL));
+    TRY(launch_bwd_gemm(s, st, gw, NL));
   }
   // ---- 4. cell weight and bias gradients over all steps; layer-0 input rows
   for (int side = 0; side < 2; ++side) {
@@ -947,25 +921,20 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
       x.h0_rows = N; x.ldh = L; x.kh = L;
       x.G = dgates_at(s, side, l, 0, N); x.ldg = L4; x.C = L4; x.R = R;
       x.out = off(cell_prefix(side, l) + "weights"); x.ldo = L4;
-      if ((rc = launch_xtb(s, st, x))) return rc;
-      if ((rc = launch_colsum(s, st, dgates_at(s, side, l, 0, N), R, L4, L4,
-                              off(cell_prefix(side, l) + "biases"))))
-        return rc;
+      TRY(launch_xtb(s, st, x));
+      TRY(launch_colsum(s, st, dgates_at(s, side, l, 0, N), R, L4, L4,
+                        off(cell_prefix(side, l) + "biases")));
     }
     // embedding rows: d x0 = dgates · W_xᵀ, scattered into the looked-up rows
-    rc = one_gemm(s, st, bwd_gemm(gemm_ops(dgates_at(s, side, 0, 0, N), L4, R, L4, s->w_t[side][0],
-                                           in_dim(side, 0) + L, in_dim(side, 0)),
-                                  s->dx0, in_dim(side, 0), nullptr, 0, in_dim(side, 0), false));
-    if (rc) return rc;
+    TRY(one_gemm(s, st, bwd_gemm(gemm_ops(dgates_at(s, side, 0, 0, N), L4, R, L4, s->w_t[side][0],
+                                          in_dim(side, 0) + L, in_dim(side, 0)),
+                                 s->dx0, in_dim(side, 0), nullptr, 0, in_dim(side, 0), false)));
     if (side == 0)
-      s2s_scatter_rows_kernel<<<R, 128, 0, st>>>(s->dx0, Et, s->rec_seq, 0, 0,
-                                                  off("encoder/embedding_mat"), g.num_vocab_txt, nullptr);
+      TRY(launch(s->launches, s2s_scatter_rows_kernel, R, 128, 0, st, {}, s->dx0, Et, s->rec_seq, 0,
+                 0, off("encoder/embedding_mat"), g.num_vocab_txt, nullptr));
     else
-      s2s_scatter_rows_kernel<<<R, 128, 0, st>>>(s->dx0, En, s->rec_tok, N, Vn,
-                                                  off("decoder/embedding_mat"), Vn,
-                                                  off("decoder/go_embedding"));
-    ++s->launches;
-    S2S_TRY(cudaGetLastError());
+      TRY(launch(s->launches, s2s_scatter_rows_kernel, R, 128, 0, st, {}, s->dx0, En, s->rec_tok, N,
+                 Vn, off("decoder/embedding_mat"), Vn, off("decoder/go_embedding")));
   }
   return N2NMN_OK;
 }
@@ -987,15 +956,37 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
     return fail_with(N2NMN_ERR_ARG,
                      "bad seq2seq config (lstm_dim must be a multiple of 8, embed dims of 4, num_vocab_nmn <= 64, "
                      "num_layers <= 4, T_encoder <= 128)");
-  S2S_TRY(cudaSetDevice(cfg->device));
+  CUDA_TRY(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
-  S2S_TRY(cudaGetDeviceProperties(&prop, cfg->device));
+  CUDA_TRY(cudaGetDeviceProperties(&prop, cfg->device));
   if (prop.major != 9)
     return fail_with(N2NMN_ERR_DEVICE, std::string("n2nmn_b200 needs an sm_90 GPU, found sm_") +
                                            std::to_string(prop.major) + std::to_string(prop.minor));
-  if (head_bwd_smem_floats(L, cfg->T_encoder) * sizeof(float) > prop.sharedMemPerBlockOptin)
+  const size_t smem_max = prop.sharedMemPerBlockOptin;
+  if (head_bwd_smem_floats(L, cfg->T_encoder) * sizeof(float) > smem_max)
     return fail_with(N2NMN_ERR_ARG, "lstm_dim too large for the backward head kernel's shared memory");
-  auto* s = new n2nmn_seq2seq;
+  const size_t attn_bytes = attn_smem_floats(L, cfg->T_encoder, cfg->num_vocab_nmn) * sizeof(float);
+  if (attn_bytes > 200 * 1024 || attn_bytes > smem_max)
+    return fail_with(N2NMN_ERR_ARG, "num_vocab_nmn * lstm_dim too large for the decoder step kernel");
+  // Kernel attributes belong to the process, not the context, so every context sets the same
+  // values: the mma_tile kernels' fixed sizes, and the device's limit for dec_attn and the head
+  // backward, whose size follows the config (checked above; neither has static shared memory).
+  for (bool exact : {false, true})
+    for (bool narrow : {false, true}) {
+      TRY(set_smem(gemm_variant(narrow, exact), (int)mma_smem_bytes(narrow ? 2 : 4)));
+      TRY(set_smem(bwd_gemm_variant(narrow, exact), (int)mma_smem_bytes(narrow ? 2 : 4)));
+      for (bool shared_sm : {false, true})
+        for (bool rec : {false, true})
+          TRY(set_smem(lstm_variant(narrow, shared_sm, exact, rec), (int)lstm_smem(narrow, shared_sm),
+                       narrow && shared_sm ? 100 : -1));
+    }
+  for (bool rec : {false, true})
+    TRY(set_smem(rec ? &dec_attn_kernel<true> : &dec_attn_kernel<false>, (int)smem_max));
+  TRY(set_smem(s2s_head_bwd_kernel, (int)smem_max));
+  // every failure below frees what was built so far (n2nmn_seq2seq_destroy takes a partial context)
+  std::unique_ptr<n2nmn_seq2seq, decltype(&n2nmn_seq2seq_destroy)> owner(new n2nmn_seq2seq,
+                                                                          n2nmn_seq2seq_destroy);
+  n2nmn_seq2seq* s = owner.get();
   s->cfg = *cfg;
   s->num_sms = prop.multiProcessorCount;
   const int C = 4 * L, N = cfg->max_batch, Vt = cfg->num_vocab_txt, Vn = cfg->num_vocab_nmn;
@@ -1028,78 +1019,41 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
     v.offset = s->flat_size;
     s->flat_size += (int64_t)((v.count + 3) & ~size_t(3));
   }
-  S2S_TRY(dmalloc(&s->wstore, (size_t)s->flat_size));
-  S2S_TRY(cudaMemset(s->wstore, 0, sizeof(float) * s->flat_size));
+  CUDA_TRY(dmalloc(s, &s->wstore, (size_t)s->flat_size));
+  CUDA_TRY(cudaMemset(s->wstore, 0, sizeof(float) * s->flat_size));
   for (auto& v : s->vars) v.dev = s->wstore + v.offset;
-  S2S_TRY(dmalloc(&s->table_enc, (size_t)Vt * C));
-  S2S_TRY(dmalloc(&s->table_dec, (size_t)(Vn + 1) * C));
-  S2S_TRY(dmalloc(&s->dec_rows, (size_t)(Vn + 1) * En));
-  S2S_TRY(dmalloc(&s->wy_t, (size_t)Vn * 2 * L));
+  CUDA_TRY(dmalloc(s, &s->table_enc, (size_t)Vt * C));
+  CUDA_TRY(dmalloc(s, &s->table_dec, (size_t)(Vn + 1) * C));
+  CUDA_TRY(dmalloc(s, &s->dec_rows, (size_t)(Vn + 1) * En));
+  CUDA_TRY(dmalloc(s, &s->wy_t, (size_t)Vn * 2 * L));
   for (int side = 0; side < 2; ++side)
     for (int l = 0; l < cfg->num_layers; ++l) {
       const int in = l == 0 ? (side == 0 ? Et : En) : L;
-      S2S_TRY(dmalloc(&s->w_cell[side][l], (size_t)(in + L) * C));
-      S2S_TRY(dmalloc(&s->b_cell[side][l], (size_t)C));
+      CUDA_TRY(dmalloc(s, &s->w_cell[side][l], (size_t)(in + L) * C));
+      CUDA_TRY(dmalloc(s, &s->b_cell[side][l], (size_t)C));
     }
   for (int l = 0; l < cfg->num_layers; ++l) {
-    S2S_TRY(dmalloc(&s->h[l][0], (size_t)N * L));
-    S2S_TRY(dmalloc(&s->h[l][1], (size_t)N * L));
-    S2S_TRY(dmalloc(&s->c[l], (size_t)N * L));
+    CUDA_TRY(dmalloc(s, &s->h[l][0], (size_t)N * L));
+    CUDA_TRY(dmalloc(s, &s->h[l][1], (size_t)N * L));
+    CUDA_TRY(dmalloc(s, &s->c[l], (size_t)N * L));
   }
   const size_t TNL = (size_t)cfg->T_encoder * N * L;
-  S2S_TRY(dmalloc(&s->enc_out, TNL));
-  S2S_TRY(dmalloc(&s->enc_ht, TNL));
-  S2S_TRY(dmalloc(&s->q, (size_t)N * L));
-  S2S_TRY(dmalloc(&s->atts, (size_t)cfg->T_decoder * cfg->T_encoder * N));
-  S2S_TRY(dmalloc(&s->X, (size_t)N * 3));
-  S2S_TRY(dmalloc(&s->cur_tok, (size_t)N));
-  S2S_TRY(dmalloc(&s->P, (size_t)Vn * 3));
-  S2S_TRY(dmalloc(&s->W, (size_t)3 * Vn * 4));
-  S2S_TRY(dmalloc(&s->b, (size_t)Vn * 4));
-  auto opt_in = [](auto kernel, size_t bytes) {
-    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  };
-  S2S_TRY(opt_in(s2s_gemm_kernel<2, true>, mma_smem_bytes(2)));
-  S2S_TRY(opt_in(s2s_gemm_kernel<2, false>, mma_smem_bytes(2)));
-  S2S_TRY(opt_in(s2s_gemm_kernel<4, true>, mma_smem_bytes(4)));
-  S2S_TRY(opt_in(s2s_gemm_kernel<4, false>, mma_smem_bytes(4)));
-  S2S_TRY(opt_in(lstm_step_kernel<2, true, 5>, mma_smem_bytes(2, 5)));
-  S2S_TRY(opt_in(lstm_step_kernel<2, false, 5>, mma_smem_bytes(2, 5)));
-  S2S_TRY(opt_in(lstm_step_kernel<2, true, 3>, mma_smem_bytes(2, 3)));
-  S2S_TRY(opt_in(lstm_step_kernel<2, false, 3>, mma_smem_bytes(2, 3)));
-  S2S_TRY(opt_in(lstm_step_kernel<4, true, 3>, mma_smem_bytes(4, 3)));
-  S2S_TRY(opt_in(lstm_step_kernel<4, false, 3>, mma_smem_bytes(4, 3)));
-  S2S_TRY(cudaFuncSetAttribute(lstm_step_kernel<2, true, 3>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  S2S_TRY(cudaFuncSetAttribute(lstm_step_kernel<2, false, 3>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  const size_t attn_bytes = attn_smem_floats(L, cfg->T_encoder, Vn) * sizeof(float);
-  if (attn_bytes > 200 * 1024 || attn_bytes > prop.sharedMemPerBlockOptin)
-    return fail_with(N2NMN_ERR_ARG, "num_vocab_nmn * lstm_dim too large for the decoder step kernel");
-  S2S_TRY(cudaFuncSetAttribute(dec_attn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)attn_bytes));
-  *out = s;
+  CUDA_TRY(dmalloc(s, &s->enc_out, TNL));
+  CUDA_TRY(dmalloc(s, &s->enc_ht, TNL));
+  CUDA_TRY(dmalloc(s, &s->q, (size_t)N * L));
+  CUDA_TRY(dmalloc(s, &s->atts, (size_t)cfg->T_decoder * cfg->T_encoder * N));
+  CUDA_TRY(dmalloc(s, &s->X, (size_t)N * 3));
+  CUDA_TRY(dmalloc(s, &s->cur_tok, (size_t)N));
+  CUDA_TRY(dmalloc(s, &s->P, (size_t)Vn * 3));
+  CUDA_TRY(dmalloc(s, &s->W, (size_t)3 * Vn * 4));
+  CUDA_TRY(dmalloc(s, &s->b, (size_t)Vn * 4));
+  *out = owner.release();
   return N2NMN_OK;
 }
 
 int n2nmn_seq2seq_destroy(n2nmn_seq2seq* s) {
   if (!s) return N2NMN_OK;
-  cudaFree(s->wstore);
-  for (int side = 0; side < 2; ++side) {
-    cudaFree(s->rec_gates[side]); cudaFree(s->rec_c[side]); cudaFree(s->rec_h[side]);
-    cudaFree(s->dgates[side]);
-    for (int l = 0; l < kMaxLayers; ++l) cudaFree(s->w_t[side][l]);
-  }
-  cudaFree(s->rec_q); cudaFree(s->rec_d2); cudaFree(s->rec_sc); cudaFree(s->rec_att);
-  cudaFree(s->rec_valid_bits); cudaFree(s->rec_tok); cudaFree(s->rec_seq); cudaFree(s->rec_len);
-  for (auto* p : s->d_h) cudaFree(p);
-  cudaFree(s->ds); cudaFree(s->dh_top); cudaFree(s->dq); cudaFree(s->dv_part);
-  cudaFree(s->d_enc_out); cudaFree(s->d_enc_ht); cudaFree(s->dx0);
-  cudaFree(s->wa_t); cudaFree(s->wh_t); cudaFree(s->d_segs); cudaFree(s->d_sumsq);
-  cudaFree(s->table_enc); cudaFree(s->table_dec); cudaFree(s->dec_rows); cudaFree(s->wy_t);
-  for (int side = 0; side < 2; ++side)
-    for (int l = 0; l < kMaxLayers; ++l) { cudaFree(s->w_cell[side][l]); cudaFree(s->b_cell[side][l]); }
-  for (int l = 0; l < kMaxLayers; ++l) { cudaFree(s->h[l][0]); cudaFree(s->h[l][1]); cudaFree(s->c[l]); }
-  cudaFree(s->enc_out); cudaFree(s->enc_ht); cudaFree(s->q); cudaFree(s->atts);
-  cudaFree(s->X); cudaFree(s->cur_tok); cudaFree(s->P); cudaFree(s->W); cudaFree(s->b);
+  for (void* p : s->allocs) cudaFree(p);
   delete s;
   return N2NMN_OK;
 }
@@ -1125,8 +1079,8 @@ int n2nmn_seq2seq_set_weight(n2nmn_seq2seq* s, const char* name, const float* sr
   bool same = ndim == (int)v.shape.size();
   for (int d = 0; same && d < ndim; ++d) same = shape[d] == v.shape[d];
   if (!same) return fail_with(N2NMN_ERR_ARG, std::string("shape mismatch for ") + name);
-  S2S_TRY(cudaMemcpyAsync(v.dev, src_dev, v.count * sizeof(float), cudaMemcpyDeviceToDevice,
-                          (cudaStream_t)stream));
+  CUDA_TRY(cudaMemcpyAsync(v.dev, src_dev, v.count * sizeof(float), cudaMemcpyDeviceToDevice,
+                           (cudaStream_t)stream));
   v.loaded = true;
   s->dirty = true;
   s->bwd_dirty = true;
@@ -1139,10 +1093,10 @@ int n2nmn_seq2seq_set_assembler(n2nmn_seq2seq* s, const int32_t* P, const int32_
   if (!s || !P || !W || !b) return fail_with(N2NMN_ERR_ARG, "null argument");
   const int Vn = s->cfg.num_vocab_nmn;
   auto st = (cudaStream_t)stream;
-  S2S_TRY(cudaMemcpyAsync(s->P, P, sizeof(int32_t) * Vn * 3, cudaMemcpyHostToDevice, st));
-  S2S_TRY(cudaMemcpyAsync(s->W, W, sizeof(int32_t) * 3 * Vn * 4, cudaMemcpyHostToDevice, st));
-  S2S_TRY(cudaMemcpyAsync(s->b, b, sizeof(int32_t) * Vn * 4, cudaMemcpyHostToDevice, st));
-  S2S_TRY(cudaStreamSynchronize(st));   // the host arrays may be temporaries
+  CUDA_TRY(cudaMemcpyAsync(s->P, P, sizeof(int32_t) * Vn * 3, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(s->W, W, sizeof(int32_t) * 3 * Vn * 4, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(s->b, b, sizeof(int32_t) * Vn * 4, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaStreamSynchronize(st));   // the host arrays may be temporaries
   s->tables_set = true;
   return N2NMN_OK;
 }
@@ -1172,27 +1126,19 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
   auto st = (cudaStream_t)stream;
   s->rec_valid = false;
   const bool rec = s->record;
-  if (rec) {
-    const int rc = ensure_record(s);
-    if (rc) return rc;
-  }
-  if (s->dirty) {
-    const int rc = prepare(s, st);
-    if (rc) return rc;
-  }
+  if (rec) TRY(ensure_record(s));
+  if (s->dirty) TRY(prepare(s, st));
   const int L = g.lstm_dim, C = 4 * L, NL = g.num_layers, Vn = g.num_vocab_nmn;
   const int Et = g.embed_dim_txt, En = g.embed_dim_nmn, T_dec = g.T_decoder;
   float* atts = atts_dev ? atts_dev : s->atts;
   for (int l = 0; l < NL; ++l) {
-    S2S_TRY(cudaMemsetAsync(s->h[l][0], 0, sizeof(float) * N * L, st));
-    S2S_TRY(cudaMemsetAsync(s->c[l], 0, sizeof(float) * N * L, st));
+    CUDA_TRY(cudaMemsetAsync(s->h[l][0], 0, sizeof(float) * N * L, st));
+    CUDA_TRY(cudaMemsetAsync(s->c[l], 0, sizeof(float) * N * L, st));
   }
-  init_state_kernel<<<(N + 127) / 128, 128, 0, st>>>(s->X, s->cur_tok, neg_entropy_dev, N, T_dec, Vn);
-  ++s->launches;
-  const bool narrow = narrow_tiles(C / kMmaCols, N, s->num_sms);
-  const dim3 grid(C / kMmaCols, narrow ? (N + 31) / 32 : (N + 63) / 64);
+  TRY(launch(s->launches, init_state_kernel, (N + 127) / 128, 128, 0, st, {}, s->X, s->cur_tok,
+             neg_entropy_dev, N, T_dec, Vn));
+  const Tiles tl = tiles(N, C, 1, s->num_sms);
   int cur = 0;   // h[l][cur] holds every layer's h_{t-1}
-  bool ok = true;
   const bool exact = !(g.flags & N2NMN_SEQ2SEQ_FLAG_TF32);
   // one LSTM cell evaluation: layer l of `side` at step t; `par` = parity of the h buffer that
   // holds the layer's previous state (its own and the layer below's run in lock step)
@@ -1217,31 +1163,9 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     return p;
   };
   auto launch_wave = [&](const LstmWave& w, int nz, bool shared_sm) {
-    const dim3 g3(grid.x, grid.y, nz), blk(kMmaThreads);
-    cudaError_t le;
-    if (rec) {
-      if (!narrow) {
-        le = exact ? launch(lstm_step_kernel<4, true, 3, true>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w)
-                   : launch(lstm_step_kernel<4, false, 3, true>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w);
-      } else if (shared_sm) {
-        le = exact ? launch(lstm_step_kernel<2, true, 3, true>, g3, blk, mma_smem_bytes(2, 3), st, kPdl, w)
-                   : launch(lstm_step_kernel<2, false, 3, true>, g3, blk, mma_smem_bytes(2, 3), st, kPdl, w);
-      } else {
-        le = exact ? launch(lstm_step_kernel<2, true, 5, true>, g3, blk, mma_smem_bytes(2, 5), st, kPdl, w)
-                   : launch(lstm_step_kernel<2, false, 5, true>, g3, blk, mma_smem_bytes(2, 5), st, kPdl, w);
-      }
-    } else if (!narrow) {
-      le = exact ? launch(lstm_step_kernel<4, true, 3>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w)
-                 : launch(lstm_step_kernel<4, false, 3>, g3, blk, mma_smem_bytes(4, 3), st, kPdl, w);
-    } else if (shared_sm) {
-      le = exact ? launch(lstm_step_kernel<2, true, 3>, g3, blk, mma_smem_bytes(2, 3), st, kPdl, w)
-                 : launch(lstm_step_kernel<2, false, 3>, g3, blk, mma_smem_bytes(2, 3), st, kPdl, w);
-    } else {
-      le = exact ? launch(lstm_step_kernel<2, true, 5>, g3, blk, mma_smem_bytes(2, 5), st, kPdl, w)
-                 : launch(lstm_step_kernel<2, false, 5>, g3, blk, mma_smem_bytes(2, 5), st, kPdl, w);
-    }
-    if (le != cudaSuccess) ok = false;
-    ++s->launches;
+    return launch(s->launches, lstm_variant(tl.narrow, shared_sm, exact, rec),
+                  dim3(tl.grid.x, tl.grid.y, nz), kMmaThreads, lstm_smem(tl.narrow, shared_sm), st,
+                  kPdl, w);
   };
   // encoder, dynamic_rnn (:95-99): tick k runs layer l at step t = k - l
   for (int k = 0; k < T_enc + NL - 1; ++k) {
@@ -1253,7 +1177,7 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
       w.s[l] = cell(0, l, t, t & 1, input_seq_dev + (size_t)t * N, seq_len_dev,
                     s->enc_out + (size_t)t * N * L);
     }
-    launch_wave(w, NL, NL > 1);
+    TRY(launch_wave(w, NL, NL > 1));
   }
   cur = T_enc & 1;
   // dynamic_rnn's final state (:95-99), (c, h) per layer: the decoder's initial state, which its
@@ -1261,32 +1185,26 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
   if (encoder_states_dev != nullptr)
     for (int l = 0; l < NL; ++l) {
       float* dst = encoder_states_dev + (size_t)l * 2 * N * L;
-      S2S_TRY(cudaMemcpyAsync(dst, s->c[l], sizeof(float) * N * L, cudaMemcpyDeviceToDevice, st));
-      S2S_TRY(cudaMemcpyAsync(dst + (size_t)N * L, s->h[l][cur], sizeof(float) * N * L,
-                              cudaMemcpyDeviceToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(dst, s->c[l], sizeof(float) * N * L, cudaMemcpyDeviceToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(dst + (size_t)N * L, s->h[l][cur], sizeof(float) * N * L,
+                               cudaMemcpyDeviceToDevice, st));
     }
-  // decoder step: the layers of one step depend on each other, one launch each
-  auto step = [&](int t, const int32_t* tok) {
+  TRY(launch_gemm(s, st, s->enc_out, L, T_enc * N, L, s->v("encoder/encoder_h_transform/weights"),
+                  L, L, s->v("encoder/encoder_h_transform/biases"), s->enc_ht, L));   // :104-108
+  const size_t attn_smem = attn_smem_floats(L, T_enc, Vn) * sizeof(float);
+  for (int t = 0; t < T_dec; ++t) {   // raw_rnn loop (:199-305)
+    // decoder step: the layers of one step depend on each other, one launch each
     for (int l = 0; l < NL; ++l) {
       LstmWave w;
       std::memset(&w, 0, sizeof(w));
-      w.s[0] = cell(1, l, t, cur, tok, nullptr, nullptr);
-      launch_wave(w, 1, false);
+      w.s[0] = cell(1, l, t, cur, s->cur_tok, nullptr, nullptr);
+      TRY(launch_wave(w, 1, false));
     }
     cur ^= 1;
-  };
-  S2S_TRY(cudaGetLastError());
-  int rc = launch_gemm(s, st, s->enc_out, L, T_enc * N, L, s->v("encoder/encoder_h_transform/weights"),
-                       L, L, s->v("encoder/encoder_h_transform/biases"), s->enc_ht, L);   // :104-108
-  if (rc) return rc;
-  const size_t attn_smem = attn_smem_floats(L, T_enc, Vn) * sizeof(float);
-  for (int t = 0; t < T_dec; ++t) {   // raw_rnn loop (:199-305)
-    step(t, s->cur_tok);
     const float* h_top = s->h[NL - 1][cur];
     float* q = rec ? s->rec_q + (size_t)t * N * L : s->q;   // the recording keeps every query
-    rc = launch_gemm(s, st, h_top, L, N, L, s->v("decoder/att_prediction/weights"), L, L,
-                     s->v("decoder/att_prediction/biases"), q, L);
-    if (rc) return rc;
+    TRY(launch_gemm(s, st, h_top, L, N, L, s->v("decoder/att_prediction/weights"), L, L,
+                    s->v("decoder/att_prediction/biases"), q, L));
     AttnStep a;
     a.q = q; a.h_top = h_top; a.enc_ht = s->enc_ht; a.enc_out = s->enc_out;
     a.v = s->v("decoder/att_prediction/v");
@@ -1305,21 +1223,15 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     a.rec_att = rec ? s->rec_att + (size_t)t * T_enc * N : nullptr;
     a.rec_valid = rec ? s->rec_valid_bits + (size_t)t * N * 2 : nullptr;
     a.rec_tok = rec ? s->rec_tok + (size_t)t * N : nullptr;
-    if ((rec ? launch(dec_attn_kernel<true>, dim3(N), dim3(kAttnThreads), attn_smem, st, kPdl, a)
-             : launch(dec_attn_kernel<false>, dim3(N), dim3(kAttnThreads), attn_smem, st, kPdl, a)) !=
-        cudaSuccess)
-      ok = false;
-    ++s->launches;
+    TRY(launch(s->launches, rec ? &dec_attn_kernel<true> : &dec_attn_kernel<false>, N, kAttnThreads,
+               attn_smem, st, kPdl, a));
   }
-  word_vecs_kernel<<<dim3(N, T_dec), 128, sizeof(float) * 2 * T_enc, st>>>(
-      atts, input_seq_dev, s->v("encoder/embedding_mat"), word_vecs_dev, T_enc, N, Et);
-  ++s->launches;
-  S2S_TRY(cudaGetLastError());
-  if (!ok) return fail_with(N2NMN_ERR_CUDA, "seq2seq kernel launch failed");
+  TRY(launch(s->launches, word_vecs_kernel, dim3(N, T_dec), 128, sizeof(float) * 2 * T_enc, st, {},
+             atts, input_seq_dev, s->v("encoder/embedding_mat"), word_vecs_dev, T_enc, N, Et));
   if (rec) {   // the inputs may be temporaries of the caller
-    S2S_TRY(cudaMemcpyAsync(s->rec_seq, input_seq_dev, sizeof(int32_t) * T_enc * N,
-                            cudaMemcpyDeviceToDevice, st));
-    S2S_TRY(cudaMemcpyAsync(s->rec_len, seq_len_dev, sizeof(int32_t) * N, cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(s->rec_seq, input_seq_dev, sizeof(int32_t) * T_enc * N,
+                             cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(s->rec_len, seq_len_dev, sizeof(int32_t) * N, cudaMemcpyDeviceToDevice, st));
     s->rec_N = N;
     s->rec_T = T_enc;
     s->rec_valid = true;
@@ -1372,8 +1284,8 @@ int n2nmn_seq2seq_backward_ex(n2nmn_seq2seq* s, const float* d_log_seq_prob_dev,
 
 int n2nmn_seq2seq_load_flat_weights(n2nmn_seq2seq* s, const float* wflat_dev, void* stream) {
   if (!s || !wflat_dev) return fail_with(N2NMN_ERR_ARG, "null argument");
-  S2S_TRY(cudaMemcpyAsync(s->wstore, wflat_dev, sizeof(float) * s->flat_size,
-                          cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  CUDA_TRY(cudaMemcpyAsync(s->wstore, wflat_dev, sizeof(float) * s->flat_size,
+                           cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   for (auto& v : s->vars) v.loaded = true;
   s->dirty = true;
   s->bwd_dirty = true;
@@ -1383,8 +1295,8 @@ int n2nmn_seq2seq_load_flat_weights(n2nmn_seq2seq* s, const float* wflat_dev, vo
 
 int n2nmn_seq2seq_get_flat_weights(const n2nmn_seq2seq* s, float* wflat_dev, void* stream) {
   if (!s || !wflat_dev) return fail_with(N2NMN_ERR_ARG, "null argument");
-  S2S_TRY(cudaMemcpyAsync(wflat_dev, s->wstore, sizeof(float) * s->flat_size,
-                          cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  CUDA_TRY(cudaMemcpyAsync(wflat_dev, s->wstore, sizeof(float) * s->flat_size,
+                           cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return N2NMN_OK;
 }
 
@@ -1403,22 +1315,20 @@ int n2nmn_seq2seq_adam_step(n2nmn_seq2seq* s, float* wflat_dev, float* gflat_dev
       const std::string& n = s->vars[i].name;   // l2_reg covers ".../weights" only (nmn3_model.py:161-166)
       segs[i].decay = n.size() >= 8 && n.compare(n.size() - 8, 8, "/weights") == 0;
     }
-    S2S_TRY(dmalloc_once(&s->d_segs, (size_t)nv));
-    S2S_TRY(cudaMemcpy(s->d_segs, segs.data(), nv * sizeof(VarSeg), cudaMemcpyHostToDevice));
-    S2S_TRY(dmalloc_once(&s->d_sumsq, (size_t)nv));
+    CUDA_TRY(dmalloc_once(s, &s->d_segs, (size_t)nv));
+    CUDA_TRY(cudaMemcpy(s->d_segs, segs.data(), nv * sizeof(VarSeg), cudaMemcpyHostToDevice));
+    CUDA_TRY(dmalloc_once(s, &s->d_sumsq, (size_t)nv));
     s->segs_ready = true;
   }
-  S2S_TRY(cudaMemsetAsync(s->d_sumsq, 0, nv * sizeof(float), st));
+  CUDA_TRY(cudaMemsetAsync(s->d_sumsq, 0, nv * sizeof(float), st));
   const dim3 grid(32, nv);
-  grad_norm_kernel<<<grid, 256, 0, st>>>(wflat_dev, gflat_dev, s->d_segs, weight_decay, 1.f,
-                                         s->d_sumsq, nullptr);
+  TRY(launch(s->launches, grad_norm_kernel, grid, 256, 0, st, {}, wflat_dev, gflat_dev, s->d_segs,
+             weight_decay, 1.f, s->d_sumsq, nullptr));
   const double lr_t = (double)lr * std::sqrt(1.0 - std::pow((double)beta2, step)) /
                       (1.0 - std::pow((double)beta1, step));
-  adam_clip_kernel<false><<<grid, 256, 0, st>>>(wflat_dev, gflat_dev, m_dev, v_dev, s->d_segs,
-                                                s->d_sumsq, (float)lr_t, beta1, beta2, eps, max_norm,
-                                                nullptr, nullptr, 0);
-  s->launches += 2;
-  S2S_TRY(cudaGetLastError());
+  TRY(launch(s->launches, adam_clip_kernel<false>, grid, 256, 0, st, {}, wflat_dev, gflat_dev,
+             m_dev, v_dev, s->d_segs, s->d_sumsq, (float)lr_t, beta1, beta2, eps, max_norm,
+             nullptr, nullptr, 0));
   return n2nmn_seq2seq_load_flat_weights(s, wflat_dev, stream);
 }
 

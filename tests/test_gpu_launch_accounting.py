@@ -3,7 +3,8 @@
 For fixed seeded workloads, how many kernels each entry point launches (n2nmn_launch_count) and
 which profile regions it records (n2nmn_set_profiling / n2nmn_get_launch_times) are pinned: the
 benchmark's kernel pass keys on those region names, and the counts show a launch that went missing
-or was added. A failed n2nmn_create must free everything it allocated before it failed."""
+or was added. A failed n2nmn_create or n2nmn_seq2seq_create must free everything it allocated
+before it failed."""
 import ctypes as C
 
 import numpy as np
@@ -143,3 +144,24 @@ def test_failed_create_frees_its_allocations():
     torch.cuda.synchronize()
     free1, _ = torch.cuda.mem_get_info()
     assert free0 - free1 < 256 << 20, (free0 - free1) / 2**20
+
+
+def test_failed_seq2seq_create_frees_its_allocations():
+    """A 64-token layout vocabulary at lstm_dim 512 needs about 284 KB of shared memory in the
+    decoder step kernel: refused, with nothing left allocated (a context of this size holds about
+    240 MB, most of it the 17,742-row input table of the question vocabulary)."""
+    lib = _lib.lib()
+    cfg = _lib.Seq2SeqConfig(abi_version=_lib.ABI_VERSION, num_vocab_txt=17742, embed_dim_txt=300,
+                             num_vocab_nmn=64, embed_dim_nmn=300, lstm_dim=512, num_layers=2,
+                             T_encoder=45, T_decoder=10, max_batch=64,
+                             device=torch.cuda.current_device(), flags=0)
+    torch.cuda.synchronize()
+    free0, _ = torch.cuda.mem_get_info()
+    for _ in range(5):
+        h = C.c_void_p()
+        assert lib.n2nmn_seq2seq_create(C.byref(cfg), C.byref(h)) == -1   # N2NMN_ERR_ARG
+        assert b'decoder step kernel' in lib.n2nmn_last_error()
+        assert not h.value
+    torch.cuda.synchronize()
+    free1, _ = torch.cuda.mem_get_info()
+    assert free0 - free1 < 64 << 20, (free0 - free1) / 2**20

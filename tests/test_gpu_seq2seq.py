@@ -159,6 +159,35 @@ def test_single_pass_tf32_option_stays_within_1e_3():
     check(out, *decf, atol=2e-3)
 
 
+def test_generators_of_different_sizes_coexist():
+    """Kernel attributes belong to the process: creating and running a generator of a smaller
+    lstm_dim must not lower the shared memory limit an earlier, larger one launches with (plain
+    and recording forwards, backward)."""
+    asm = Assembler(synth.vocab_file('clevr'))
+    N, T_enc, T_dec, V_txt, E, layers = 8, 6, 5, 30, 32, 2
+    rng = np.random.RandomState(4)
+    seq = rng.randint(0, V_txt, size=(T_enc, N)).astype(np.int32)
+    lens = rng.randint(1, T_enc + 1, size=N).astype(np.int32)
+    d_lsp = torch.ones(N, device='cuda')
+
+    def generator(L):
+        w = init_seq2seq_weights(V_txt, E, asm.num_vocab_nmn, E, L, layers, seed=L)
+        return make(asm, w, T_enc, N, T_dec, V_txt, E, E, L, layers)
+    a = generator(1000)
+    first = [o.clone() for o in a.forward(seq, lens, record=True)]
+    a.backward(d_log_seq_prob=d_lsp)
+    b = generator(512)
+    b.forward(seq, lens, record=True)
+    b.backward(d_log_seq_prob=d_lsp)
+    for record in (False, True):
+        again = a.forward(seq, lens, record=record)
+        torch.cuda.synchronize()
+        for x, y in zip(first, again):
+            assert torch.equal(x, y)
+    a.backward(d_log_seq_prob=d_lsp)
+    torch.cuda.synchronize()
+
+
 def test_errors_are_loud():
     from n2nmn_b200 import _lib
     asm = Assembler(synth.vocab_file('clevr'))

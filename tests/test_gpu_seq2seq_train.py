@@ -120,17 +120,22 @@ def test_null_upstreams():
 
 
 def test_recording_leaves_forward_bit_identical_and_launch_counts():
+    from n2nmn_b200.trainer import LayoutGeneratorTrainer
     for size in ('clevr', 'golden'):
         cfg = CFGS[size]
         N, T_enc, T_dec, V_txt, E_txt, E_nmn, L, layers = cfg
         asm, w, seq, lens = problem(cfg)
         s = make(asm, w, T_enc, N, T_dec, V_txt, E_txt, E_nmn, L, layers)
+        n_set = s.launch_count()
         a = [o.clone() for o in s.forward(seq, lens)]
         n0 = s.launch_count()
         a2 = [o.clone() for o in s.forward(seq, lens)]
         n_off = s.launch_count() - n0
         # recording off: (T_enc + layers - 1) + layers·T_dec + 2·T_dec + 3 launches, as before
         assert n_off == (T_enc + layers - 1) + layers * T_dec + 2 * T_dec + 3
+        # the first forward after set_weights also re-derives the packed weights: two regroups per
+        # cell, the two input tables and the transposed token_prediction matrix
+        assert n0 - n_set - n_off == 4 * layers + 3
         n1 = s.launch_count()
         b = [o.clone() for o in s.forward(seq, lens, record=True)]
         assert s.launch_count() - n1 == n_off
@@ -147,6 +152,11 @@ def test_recording_leaves_forward_bit_identical_and_launch_counts():
         want = 14 + 2 * layers * T_dec + 2 * (T_enc + layers - 1) + 4 * layers
         assert per == want, (per, want)
         assert first == want + 2 * layers + 2      # the transposed matrices, once per weight change
+        tr = LayoutGeneratorTrainer(s)
+        s.forward(seq, lens, record=True)
+        n4 = s.launch_count()
+        tr.step(d_log_seq_prob=torch.ones(N, device='cuda'))
+        assert s.launch_count() - n4 == per + 2    # the backward, then grad_norm and adam_clip
         print('%s: forward %d launches, backward %d' % (size, n_off, per))
 
 

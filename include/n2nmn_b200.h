@@ -383,9 +383,10 @@ int64_t n2nmn_launch_count(const n2nmn_ctx* ctx);
 
 /* ---- (f1) attentional seq2seq layout generator --------------------------------------------
  * Replaces `AttentionSeq2Seq` (models_clevr/nmn3_netgen_att.py:46-322; the VQA / SHAPES copies
- * are the same code) without dropout: greedy decoding under the Assembler's validity masks,
- * `decoder_sampling` (n2nmn_seq2seq_set_sampling) or teacher forcing: the encoder LSTM stack
- * under dynamic_rnn (:73-120) and the raw_rnn attention decoder (:122-322). Training: a recording
+ * are the same code): greedy decoding under the Assembler's validity masks, `decoder_sampling`
+ * (n2nmn_seq2seq_set_sampling) or teacher forcing, with the training scripts' LSTM dropout
+ * (`encoder_dropout` / `decoder_dropout`, n2nmn_seq2seq_set_dropout) or without it: the encoder LSTM
+ * stack under dynamic_rnn (:73-120) and the raw_rnn attention decoder (:122-322). Training: a recording
  * forward (n2nmn_seq2seq_set_record), n2nmn_seq2seq_backward into a flat gradient buffer and
  * n2nmn_seq2seq_adam_step (DESIGN.md §4c). */
 typedef struct n2nmn_seq2seq n2nmn_seq2seq;
@@ -457,6 +458,20 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
  * distribution; TF's generator itself is not reproducible outside TF) and replaced by the greedy
  * token if it is invalid (:241-256). NULL = back to greedy decoding. gt_layout_dev still wins. */
 int n2nmn_seq2seq_set_sampling(n2nmn_seq2seq* s, const float* uniforms_dev);
+/* `encoder_dropout` / `decoder_dropout` (nmn3_netgen_att.py:17-44, :91, :303) for the following
+ * forward calls: DropoutWrapper(output_keep_prob=0.5) on every layer but the top one. Only the
+ * output a layer hands to the layer above is dropped; its state (c, h), the encoder outputs, the
+ * attention and the token scores see undropped values, and with num_layers == 1 nothing changes.
+ * tf.nn.dropout's rule on given uniform numbers u in [0,1): an element is kept iff
+ * floor(0.5 + u) = 1 in fp32 (u >= 0.5 on torch.rand's grid) and a kept element is 2x; TF's
+ * generator itself is not reproducible outside TF. Device fp32 uniforms, indexed by (step, layer):
+ *   enc_uniforms_dev [T_enc][num_layers-1][N][lstm_dim], dec_uniforms_dev
+ *   [T_decoder][num_layers-1][N][lstm_dim]
+ * with the forward call's T_enc and N; they must stay valid until the forward's work has run (a
+ * recording forward keeps the keep-masks, so the backward does not read them). NULL = no dropout
+ * on that side. Same launches as without dropout. */
+int n2nmn_seq2seq_set_dropout(n2nmn_seq2seq* s, const float* enc_uniforms_dev,
+                              const float* dec_uniforms_dev);
 int64_t n2nmn_seq2seq_launch_count(const n2nmn_seq2seq* s);
 /* Recording switch for the following forward calls (default off). While on, the forward also
  * keeps what n2nmn_seq2seq_backward needs: every cell's gates and state, every decoding step's

@@ -53,6 +53,7 @@ SIGNATURES = {
     'n2nmn_seq2seq_forward_ex': (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                                            _P]),
     'n2nmn_seq2seq_set_sampling': (C.c_int, [_P, _P]),
+    'n2nmn_seq2seq_set_dropout': (C.c_int, [_P, _P, _P]),
     'n2nmn_seq2seq_launch_count': (C.c_int64, [_P]),
     'n2nmn_seq2seq_set_record': (C.c_int, [_P, C.c_int]),
     'n2nmn_seq2seq_backward': (C.c_int, [_P, _P, _P, _P, _P, _P]),

@@ -26,6 +26,8 @@
 // (weights, tables) before griddepcontrol.wait.
 // At N = 64 an LSTM launch costs the issue time of its mma.sync instructions (three passes for fp32
 // parity; DESIGN.md §4c).
+// Dropout (n2nmn_seq2seq_set_dropout): the training scripts' DropoutWrapper on the layers below the
+// top one, applied to given uniforms in the LSTM step epilogue (lstm_step_kernel's kDrop variant).
 // Training: with n2nmn_seq2seq_set_record on, the forward also stores what the backward pass
 // (n2nmn_seq2seq_backward, kernels in seq2seq_bwd.cuh) reads; n2nmn_seq2seq_adam_step runs the
 // module network's clip + Adam kernels (optim.cuh) over the flat variable layout.
@@ -116,6 +118,12 @@ struct LstmStep {
   // recording forward only (kRecord): activated gates i, j, f, o [N][4L] in TF's column order,
   // c_t and h_t [N][L] (the carried state past the sequence end)
   float *rec_gates, *rec_c, *rec_h;
+  // dropout of this layer's output (kDrop; nullptr on the top layer or with dropout off): this
+  // step's uniforms [N][L]; the dropped output [N][L] that the layer above reads as its x; the
+  // keep-mask [N][L] (recording forward only)
+  const float* drop_u;
+  float* drop_out;
+  uint8_t* drop_keep;
 };
 
 // BasicLSTMCell(forget_bias=1) step (gate order i, j, f, o) with dynamic_rnn's masking: past the
@@ -127,8 +135,11 @@ struct LstmStep {
 // N == 0 is idle) and the encoder takes T + layers - 1 launches instead of T * layers. With the
 // 3-stage ring two CTAs share an SM, which keeps as many bytes in flight as the 5-stage ring of
 // the single-step launches.
+// kDrop: DropoutWrapper(output_keep_prob=0.5) on the layers below the top (nmn3_netgen_att.py:17-44)
+// as tf.nn.dropout computes it: kept iff floor(0.5 + u) = 1 in fp32, a kept element is 2·h. Only the
+// copy the layer above reads is dropped; h_out, c, out_seq and the record keep the undropped values.
 struct LstmWave { LstmStep s[kMaxLayers]; };
-template <int WM, bool kExact, int ST, bool kRecord = false>
+template <int WM, bool kExact, int ST, bool kRecord = false, bool kDrop = false>
 __global__ void __launch_bounds__(kMmaThreads) lstm_step_kernel(const LstmWave wave) {
   pdl_trigger();
   const LstmStep& p = wave.s[blockIdx.z];
@@ -144,7 +155,7 @@ __global__ void __launch_bounds__(kMmaThreads) lstm_step_kernel(const LstmWave w
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wm = warp % WM, g = lane >> 2,
             tig = lane & 3;
   // epilogue inputs, requested as soon as the previous step is complete (they ride under the GEMM)
-  float gt[2][4][2], c_prev[2][2], h_keep[2][2];
+  float gt[2][4][2], c_prev[2][2], h_keep[2][2], du[2][2];
   bool live[2];
   auto prefetch = [&] {
     if (warp / WM != 0) return;
@@ -172,6 +183,11 @@ __global__ void __launch_bounds__(kMmaThreads) lstm_step_kernel(const LstmWave w
       const float2 hp = *reinterpret_cast<const float2*>(p.h_prev + idx);
       c_prev[hh][0] = cp.x; c_prev[hh][1] = cp.y;
       h_keep[hh][0] = hp.x; h_keep[hh][1] = hp.y;
+      if constexpr (kDrop)
+        if (p.drop_u != nullptr) {
+          const float2 u2 = *reinterpret_cast<const float2*>(p.drop_u + idx);
+          du[hh][0] = u2.x; du[hh][1] = u2.y;
+        }
     }
   };
   if (!mma_tile<WM, kExact, ST>(mma_smem, op, row0, c0, acc, prefetch)) return;
@@ -195,6 +211,14 @@ __global__ void __launch_bounds__(kMmaThreads) lstm_step_kernel(const LstmWave w
     *reinterpret_cast<float2*>(p.h_out + idx) = make_float2(h_new[0], h_new[1]);
     if (p.out_seq != nullptr)
       *reinterpret_cast<float2*>(p.out_seq + idx) = make_float2(o_new[0], o_new[1]);
+    if constexpr (kDrop)
+      if (p.drop_u != nullptr) {
+        const bool k0 = 0.5f + du[hh][0] >= 1.f, k1 = 0.5f + du[hh][1] >= 1.f;
+        *reinterpret_cast<float2*>(p.drop_out + idx) =
+            make_float2(k0 ? 2.f * h_new[0] : 0.f, k1 ? 2.f * h_new[1] : 0.f);
+        if constexpr (kRecord)
+          *reinterpret_cast<uchar2*>(p.drop_keep + idx) = make_uchar2(k0 ? 1 : 0, k1 ? 1 : 0);
+      }
     if constexpr (kRecord) {
       const size_t gi0 = (size_t)n * C + (c0 >> 2) + 2 * tig;
       float2 act[4];
@@ -522,6 +546,9 @@ struct n2nmn_seq2seq {
   std::vector<S2SVar> vars;
   bool dirty = true, tables_set = false;
   const float* sample_u = nullptr;   // [T_decoder][N] uniforms of the following forward calls
+  // dropout uniforms of the following forward calls (n2nmn_seq2seq_set_dropout), per side
+  // [T][layers-1][N][L]; nullptr = no dropout on that side
+  const float* drop_u[2] = {};
   // derived weights
   float *table_enc = nullptr, *table_dec = nullptr, *dec_rows = nullptr;   // dec_rows = [emb; go]
   float* w_cell[2][kMaxLayers] = {};   // interleaved full matrices [(in+L)][4L]
@@ -545,6 +572,13 @@ struct n2nmn_seq2seq {
   float *rec_gates[2] = {}, *rec_c[2] = {}, *rec_h[2] = {};   // [layers][T_cap][N][4L | L]
   float *rec_q = nullptr, *rec_d2 = nullptr, *rec_sc = nullptr, *rec_att = nullptr;
   int32_t *rec_valid_bits = nullptr, *rec_tok = nullptr, *rec_seq = nullptr, *rec_len = nullptr;
+  // dropout (allocated on first use): the dropped outputs the layer above reads, one slot per
+  // step (the encoder wavefront writes step t+1 of a layer while the layer above reads step t; the
+  // backward reads them as that layer's x), and the recording forward's keep-masks;
+  // [layers-1][T_cap][max_batch][L] each, rows [t][N] as in the recording
+  float* drop_x[2] = {};
+  uint8_t* drop_keep[2] = {};
+  bool rec_drop[2] = {};     // the recorded forward ran dropout on that side
   // backward workspace, allocated with the recording
   float *dgates[2] = {};     // [layers][T_cap][N][4L]
   float *d_h[4] = {};        // drec, dup, hcarry, dc: [layers][N][L] each
@@ -592,16 +626,22 @@ auto bwd_gemm_variant(bool narrow, bool exact) {
 }
 // 64-row tiles run the 3-stage ring; 32-row tiles the 5-stage ring, or the 3-stage one where two
 // CTAs share an SM (the encoder wavefront)
-template <bool kRec>
+template <bool kRec, bool kDrop>
 auto lstm_variant(bool narrow, bool shared_sm, bool exact) {
-  if (!narrow) return exact ? &lstm_step_kernel<4, true, 3, kRec> : &lstm_step_kernel<4, false, 3, kRec>;
-  if (shared_sm) return exact ? &lstm_step_kernel<2, true, 3, kRec> : &lstm_step_kernel<2, false, 3, kRec>;
-  return exact ? &lstm_step_kernel<2, true, 5, kRec> : &lstm_step_kernel<2, false, 5, kRec>;
+  if (!narrow)
+    return exact ? &lstm_step_kernel<4, true, 3, kRec, kDrop> : &lstm_step_kernel<4, false, 3, kRec, kDrop>;
+  if (shared_sm)
+    return exact ? &lstm_step_kernel<2, true, 3, kRec, kDrop> : &lstm_step_kernel<2, false, 3, kRec, kDrop>;
+  return exact ? &lstm_step_kernel<2, true, 5, kRec, kDrop> : &lstm_step_kernel<2, false, 5, kRec, kDrop>;
 }
-auto lstm_variant(bool narrow, bool shared_sm, bool exact, bool rec) {
-  return rec ? lstm_variant<true>(narrow, shared_sm, exact)
-             : lstm_variant<false>(narrow, shared_sm, exact);
+auto lstm_variant(bool narrow, bool shared_sm, bool exact, bool rec, bool drop) {
+  if (drop)
+    return rec ? lstm_variant<true, true>(narrow, shared_sm, exact)
+               : lstm_variant<false, true>(narrow, shared_sm, exact);
+  return rec ? lstm_variant<true, false>(narrow, shared_sm, exact)
+             : lstm_variant<false, false>(narrow, shared_sm, exact);
 }
+auto cell_bwd_variant(bool drop) { return drop ? &s2s_cell_bwd_kernel<true> : &s2s_cell_bwd_kernel<false>; }
 size_t lstm_smem(bool narrow, bool shared_sm) {
   return mma_smem_bytes(narrow ? 2 : 4, narrow && !shared_sm ? 5 : 3);
 }
@@ -682,7 +722,8 @@ float* dgates_at(n2nmn_seq2seq* s, int side, int l, int t, int N) {
   const size_t L4 = 4 * (size_t)s->cfg.lstm_dim;
   return s->dgates[side] + ((size_t)l * t_cap(s, side) * s->cfg.max_batch + (size_t)t * N) * L4;
 }
-float* rec_state_at(n2nmn_seq2seq* s, float* base, int side, int l, int t, int N) {
+template <class T>
+T* rec_state_at(n2nmn_seq2seq* s, T* base, int side, int l, int t, int N) {
   const size_t L = s->cfg.lstm_dim;
   return base + ((size_t)l * t_cap(s, side) * s->cfg.max_batch + (size_t)t * N) * L;
 }
@@ -725,6 +766,16 @@ int ensure_record(n2nmn_seq2seq* s) {
   CUDA_TRY(dmalloc_once(s, &s->wa_t, L * L));
   CUDA_TRY(dmalloc_once(s, &s->wh_t, L * L));
   s->rec_ready = true;
+  return N2NMN_OK;
+}
+
+// The dropout buffers of `side`, allocated on the first forward that drops there; the keep-masks
+// on the first such forward that records.
+int ensure_dropout(n2nmn_seq2seq* s, int side, bool rec) {
+  const auto& g = s->cfg;
+  const size_t n = (size_t)(g.num_layers - 1) * t_cap(s, side) * g.max_batch * g.lstm_dim;
+  CUDA_TRY(dmalloc_once(s, &s->drop_x[side], n));
+  if (rec) CUDA_TRY(dmalloc_once(s, &s->drop_keep[side], n));
   return N2NMN_OK;
 }
 
@@ -842,6 +893,8 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
     c.c_new = rec_state_at(s, s->rec_c[side], side, l, t, N);
     c.drec = drec + l * NLs;
     c.dup = l < NL - 1 ? dup + l * NLs : nullptr;
+    c.dup_keep = l < NL - 1 && s->rec_drop[side] ? rec_state_at(s, s->drop_keep[side], side, l, t, N)
+                                                  : nullptr;
     c.dtop = l == NL - 1 ? (side == 1 ? s->dh_top : s->d_enc_out) + (size_t)t * N * L : nullptr;
     c.hcarry = side == 0 ? hcarry + l * NLs : nullptr;
     c.dc = dc + l * NLs;
@@ -857,16 +910,16 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
                     l == 0 ? nullptr : dup + (l - 1) * NLs, L, drec + l * NLs, L, l == 0 ? 0 : in,
                     false);
   };
-  auto launch_cells = [&](const CellBwdWave& w, int nz) {
-    return launch(s->launches, s2s_cell_bwd_kernel, dim3((N * L + 255) / 256, 1, nz), 256, 0, st,
-                  kPdl, w);
+  auto launch_cells = [&](int side, const CellBwdWave& w, int nz) {
+    return launch(s->launches, cell_bwd_variant(s->rec_drop[side]), dim3((N * L + 255) / 256, 1, nz),
+                  256, 0, st, kPdl, w);
   };
   for (int t = Td - 1; t >= 0; --t)
     for (int l = NL - 1; l >= 0; --l) {
       CellBwdWave cw;
       std::memset(&cw, 0, sizeof(cw));
       cw.s[0] = cell_slot(1, l, t);
-      TRY(launch_cells(cw, 1));
+      TRY(launch_cells(1, cw, 1));
       BwdGemmWave gw;
       std::memset(&gw, 0, sizeof(gw));
       gw.s[0] = gemm_slot(1, l, t);
@@ -898,7 +951,7 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
       cw.s[l] = cell_slot(0, l, t);
       gw.s[l] = gemm_slot(0, l, t);
     }
-    TRY(launch_cells(cw, NL));
+    TRY(launch_cells(0, cw, NL));
     TRY(launch_bwd_gemm(s, st, gw, NL));
   }
   // ---- 4. cell weight and bias gradients over all steps; layer-0 input rows
@@ -912,8 +965,9 @@ int backward_impl(n2nmn_seq2seq* s, const float* dlp, const float* dne, const fl
         x.idx = side == 0 ? s->rec_seq : s->rec_tok;
         x.shift = side == 0 ? 0 : N;   // decoder step 0 reads go_embedding (row V of dec_rows)
         x.first_idx = Vn;
-      } else {
-        x.x = rec_state_at(s, s->rec_h[side], side, l - 1, 0, N); x.ldx = L;
+      } else {   // the layer below's output as this layer read it: dropped, or h
+        x.x = rec_state_at(s, s->rec_drop[side] ? s->drop_x[side] : s->rec_h[side], side, l - 1, 0, N);
+        x.ldx = L;
       }
       x.kx = in;
       x.h0 = side == 0 ? nullptr : rec_state_at(s, s->rec_h[0], 0, l, T - 1, N);
@@ -977,8 +1031,9 @@ int n2nmn_seq2seq_create(const n2nmn_seq2seq_config* cfg, n2nmn_seq2seq** out) {
       TRY(set_smem(bwd_gemm_variant(narrow, exact), (int)mma_smem_bytes(narrow ? 2 : 4)));
       for (bool shared_sm : {false, true})
         for (bool rec : {false, true})
-          TRY(set_smem(lstm_variant(narrow, shared_sm, exact, rec), (int)lstm_smem(narrow, shared_sm),
-                       narrow && shared_sm ? 100 : -1));
+          for (bool drop : {false, true})
+            TRY(set_smem(lstm_variant(narrow, shared_sm, exact, rec, drop),
+                         (int)lstm_smem(narrow, shared_sm), narrow && shared_sm ? 100 : -1));
     }
   for (bool rec : {false, true})
     TRY(set_smem(rec ? &dec_attn_kernel<true> : &dec_attn_kernel<false>, (int)smem_max));
@@ -1127,8 +1182,12 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
   s->rec_valid = false;
   const bool rec = s->record;
   if (rec) TRY(ensure_record(s));
-  if (s->dirty) TRY(prepare(s, st));
   const int L = g.lstm_dim, C = 4 * L, NL = g.num_layers, Vn = g.num_vocab_nmn;
+  // with one layer there is nothing below the top layer to drop
+  const bool drop[2] = {s->drop_u[0] != nullptr && NL > 1, s->drop_u[1] != nullptr && NL > 1};
+  for (int side = 0; side < 2; ++side)
+    if (drop[side]) TRY(ensure_dropout(s, side, rec));
+  if (s->dirty) TRY(prepare(s, st));
   const int Et = g.embed_dim_txt, En = g.embed_dim_nmn, T_dec = g.T_decoder;
   float* atts = atts_dev ? atts_dev : s->atts;
   for (int l = 0; l < NL; ++l) {
@@ -1145,8 +1204,10 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
   auto cell = [&](int side, int l, int t, int par, const int32_t* tok, const int32_t* seq_len,
                   float* out_seq) {
     const int in = l == 0 ? (side == 0 ? Et : En) : L;
+    const bool dr = drop[side] && l < NL - 1;
     LstmStep p;
-    p.x = l == 0 ? nullptr : s->h[l - 1][par ^ 1];
+    p.x = l == 0 ? nullptr
+                 : drop[side] ? rec_state_at(s, s->drop_x[side], side, l - 1, t, N) : s->h[l - 1][par ^ 1];
     p.h_prev = s->h[l][par];
     p.w = s->w_cell[side][l] + (l == 0 ? (size_t)in * C : 0);
     p.table = l == 0 ? (side == 0 ? s->table_enc : s->table_dec) : nullptr;
@@ -1160,10 +1221,13 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     p.rec_gates = rec ? rec_gates_at(s, side, l, t, N) : nullptr;
     p.rec_c = rec ? rec_state_at(s, s->rec_c[side], side, l, t, N) : nullptr;
     p.rec_h = rec ? rec_state_at(s, s->rec_h[side], side, l, t, N) : nullptr;
+    p.drop_u = dr ? s->drop_u[side] + ((size_t)t * (NL - 1) + l) * N * L : nullptr;
+    p.drop_out = dr ? rec_state_at(s, s->drop_x[side], side, l, t, N) : nullptr;
+    p.drop_keep = dr && rec ? rec_state_at(s, s->drop_keep[side], side, l, t, N) : nullptr;
     return p;
   };
-  auto launch_wave = [&](const LstmWave& w, int nz, bool shared_sm) {
-    return launch(s->launches, lstm_variant(tl.narrow, shared_sm, exact, rec),
+  auto launch_wave = [&](int side, const LstmWave& w, int nz, bool shared_sm) {
+    return launch(s->launches, lstm_variant(tl.narrow, shared_sm, exact, rec, drop[side]),
                   dim3(tl.grid.x, tl.grid.y, nz), kMmaThreads, lstm_smem(tl.narrow, shared_sm), st,
                   kPdl, w);
   };
@@ -1177,7 +1241,7 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
       w.s[l] = cell(0, l, t, t & 1, input_seq_dev + (size_t)t * N, seq_len_dev,
                     s->enc_out + (size_t)t * N * L);
     }
-    TRY(launch_wave(w, NL, NL > 1));
+    TRY(launch_wave(0, w, NL, NL > 1));
   }
   cur = T_enc & 1;
   // dynamic_rnn's final state (:95-99), (c, h) per layer: the decoder's initial state, which its
@@ -1198,7 +1262,7 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
       LstmWave w;
       std::memset(&w, 0, sizeof(w));
       w.s[0] = cell(1, l, t, cur, s->cur_tok, nullptr, nullptr);
-      TRY(launch_wave(w, 1, false));
+      TRY(launch_wave(1, w, 1, false));
     }
     cur ^= 1;
     const float* h_top = s->h[NL - 1][cur];
@@ -1234,6 +1298,8 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
     CUDA_TRY(cudaMemcpyAsync(s->rec_len, seq_len_dev, sizeof(int32_t) * N, cudaMemcpyDeviceToDevice, st));
     s->rec_N = N;
     s->rec_T = T_enc;
+    s->rec_drop[0] = drop[0];
+    s->rec_drop[1] = drop[1];
     s->rec_valid = true;
   }
   return N2NMN_OK;
@@ -1242,6 +1308,14 @@ int n2nmn_seq2seq_forward_ex(n2nmn_seq2seq* s, const int32_t* input_seq_dev,
 int n2nmn_seq2seq_set_sampling(n2nmn_seq2seq* s, const float* uniforms_dev) {
   if (!s) return fail_with(N2NMN_ERR_ARG, "null argument");
   s->sample_u = uniforms_dev;
+  return N2NMN_OK;
+}
+
+int n2nmn_seq2seq_set_dropout(n2nmn_seq2seq* s, const float* enc_uniforms_dev,
+                              const float* dec_uniforms_dev) {
+  if (!s) return fail_with(N2NMN_ERR_ARG, "null argument");
+  s->drop_u[0] = enc_uniforms_dev;
+  s->drop_u[1] = dec_uniforms_dev;
   return N2NMN_OK;
 }
 

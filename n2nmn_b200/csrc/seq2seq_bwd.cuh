@@ -165,13 +165,15 @@ __global__ void __launch_bounds__(kHeadBwdThreads) s2s_head_bwd_kernel(const Hea
 // dh = drec (next step's recurrent product) + dup (the layer above's input product) + hcarry
 // (state carried through a later step past the sequence end) + dtop (head / encoder output, live
 // rows only). Past the sequence end (encoder) the gates get nothing and dh, dc pass straight
-// through (dynamic_rnn's carry, :95-99).
+// through (dynamic_rnn's carry, :95-99). kDrop: the layer above read this layer's output through
+// dropout, so its input product reaches dh as dup·2·keep (tf.nn.dropout's gradient).
 struct CellBwd {
   const float* gates;    // [N][4L] activated i, j, f, o (TF column order)
   const float* c_prev;   // [N][L] or nullptr (zero initial state)
   const float* c_new;    // [N][L]
   const float* drec;     // [N][L]
   const float* dup;      // [N][L] or nullptr
+  const uint8_t* dup_keep;   // kDrop: [N][L] keep-mask of the dropout on this layer's output
   const float* dtop;     // [N][L] or nullptr
   float* hcarry;         // [N][L] in/out or nullptr (decoder: no carry)
   float* dc;             // [N][L] in: d c_t; out: d c_{t-1}
@@ -181,6 +183,7 @@ struct CellBwd {
 };
 struct CellBwdWave { CellBwd s[kMaxLayers]; };
 
+template <bool kDrop = false>
 __global__ void __launch_bounds__(256) s2s_cell_bwd_kernel(const CellBwdWave w) {
   pdl_trigger();
   const CellBwd& p = w.s[blockIdx.z];
@@ -192,7 +195,11 @@ __global__ void __launch_bounds__(256) s2s_cell_bwd_kernel(const CellBwdWave w) 
   const int n = i / L, u = i - n * L;
   const bool live = p.seq_len == nullptr || p.t < p.seq_len[n];
   float dh = p.drec[i];
-  if (p.dup) dh += p.dup[i];
+  if constexpr (kDrop) {
+    if (p.dup) dh += p.dup_keep[i] ? 2.f * p.dup[i] : 0.f;
+  } else {
+    if (p.dup) dh += p.dup[i];
+  }
   if (p.hcarry) dh += p.hcarry[i];
   if (p.dtop && live) dh += p.dtop[i];
   const float dcin = p.dc[i];

@@ -1,9 +1,17 @@
 """Host-side mirror of the reference's layout generator ``AttentionSeq2Seq``
 (models_clevr/nmn3_netgen_att.py:46-322; models_vqa/ and models_shapes/ carry the same file) over
-the C ABI (`n2nmn_seq2seq_*`, include/n2nmn_b200.h). Forward pass without dropout: greedy decoding
-under the Assembler's validity masks, `decoder_sampling=True` (one draw per step from the masked
-token distribution, nmn3_netgen_att.py:234-256; the uniform numbers come from `torch.rand` on the
-device or from the caller, `forward(..., sample_uniforms=)`) or teacher forcing (`use_gt_layout`).
+the C ABI (`n2nmn_seq2seq_*`, include/n2nmn_b200.h). Forward pass: greedy decoding under the
+Assembler's validity masks, `decoder_sampling=True` (one draw per step from the masked token
+distribution, nmn3_netgen_att.py:234-256; the uniform numbers come from `torch.rand` on the device
+or from the caller, `forward(..., sample_uniforms=)`) or teacher forcing (`use_gt_layout`).
+
+Dropout: `encoder_dropout` / `decoder_dropout` are the training scripts' DropoutWrapper with
+output_keep_prob 0.5 on every LSTM layer but the top one (nmn3_netgen_att.py:17-44). Only what a
+layer hands to the layer above is dropped: an element is kept iff its uniform number u satisfies
+floor(0.5 + u) = 1 in fp32 (u >= 0.5) and a kept element doubles, as tf.nn.dropout computes it. The
+states, encoder outputs, attention and token scores are undropped, and with num_layers == 1 there
+is nothing to drop. The flags are attributes read at every `forward`, so one instance trains with
+dropout and evaluates without it (the reference builds two graphs for that).
 
 The reference builds a TF graph whose placeholders are fed per batch; here the constructor takes
 the shapes (and optionally the first batch) and ``forward`` / ``__call__`` runs a batch. The
@@ -43,9 +51,7 @@ class AttentionSeq2Seq:
                  encoder_dropout=False, decoder_dropout=False, decoder_sampling=False,
                  use_gt_layout=None, gt_layout_batch=None, scope='encoder_decoder', reuse=None,
                  T_encoder=None, max_batch=None, device=None, weights=None, precision='fp32'):
-        if encoder_dropout or decoder_dropout:
-            raise NotImplementedError('dropout is a training-time option; the H100 seq2seq is the '
-                                      'inference configuration')
+        self.encoder_dropout, self.decoder_dropout = bool(encoder_dropout), bool(decoder_dropout)
         self.decoder_sampling = bool(decoder_sampling)
         self.T_decoder = int(T_decoder)
         self.encoder_num_vocab, self.encoder_embed_dim = int(num_vocab_txt), int(embed_dim_txt)
@@ -134,7 +140,7 @@ class AttentionSeq2Seq:
         self._recorded_N = None
 
     def forward(self, input_seq_batch, seq_length_batch, use_gt_layout=None, gt_layout_batch=None,
-                sample_uniforms=None, record=False, with_encoder_states=False):
+                sample_uniforms=None, record=False, with_encoder_states=False, dropout_uniforms=None):
         """input_seq_batch [T_enc, N] int, seq_length_batch [N] int (device or host);
         gt_layout_batch [T_decoder, N] with use_gt_layout truthy = teacher forcing;
         sample_uniforms [T_decoder, N] in [0, 1): the numbers the sampled decoding consumes
@@ -142,7 +148,16 @@ class AttentionSeq2Seq:
         record=True keeps what `backward` needs (same outputs, bit for bit);
         with_encoder_states=True also sets `self.encoder_states` = ((c, h) of layer 0, ...), each
         [N, lstm_dim]: the encoder's final state (nmn3_netgen_att.py:95-99), which VQA's
-        question-prior net reads. Otherwise `self.encoder_states` is None."""
+        question-prior net reads. Otherwise `self.encoder_states` is None.
+        dropout_uniforms: None or an (enc, dec) pair, each None or the uniform numbers in [0, 1) of
+        one side whose dropout flag is on, enc [T_enc, num_layers-1, N, lstm_dim] and dec
+        [T_decoder, num_layers-1, N, lstm_dim], indexed by (step, layer below the top). A side whose
+        flag is on and has no numbers given draws them with `torch.rand` on the device; numbers
+        given for a side whose flag is off raise ValueError (they would silently do nothing), as do
+        numbers of the wrong shape. Draw order
+        of one forward: the sampling uniforms (decoder_sampling), then the encoder's dropout
+        uniforms, then the decoder's, so a forward without dropout uses torch's generator as
+        before; with num_layers == 1 nothing is dropped and nothing is drawn."""
         dev = self.device
 
         def i32(x):
@@ -169,6 +184,7 @@ class AttentionSeq2Seq:
                 u = u.to(dev, torch.float32).contiguous()
                 if u.shape != (self.T_decoder, N):
                     raise ValueError('sample_uniforms must be [T_decoder, N]')
+        du = self._dropout_uniforms(dropout_uniforms, T, N)
         tokens = torch.empty((self.T_decoder, N), dtype=torch.int32, device=dev)
         probs = torch.empty((self.T_decoder, N), dtype=torch.float32, device=dev)
         ent = torch.empty((N,), dtype=torch.float32, device=dev)
@@ -182,13 +198,15 @@ class AttentionSeq2Seq:
             check(self._L.n2nmn_seq2seq_set_record(self._h, 1 if record else 0))
             check(self._L.n2nmn_seq2seq_set_sampling(
                 self._h, C.c_void_p(u.data_ptr()) if u is not None else None))
+            check(self._L.n2nmn_seq2seq_set_dropout(
+                self._h, *[C.c_void_p(d.data_ptr()) if d is not None else None for d in du]))
             check(self._L.n2nmn_seq2seq_forward_ex(
                 self._h, C.c_void_p(seq.data_ptr()), C.c_void_p(lens.data_ptr()), T, N,
                 C.c_void_p(gt.data_ptr()) if gt is not None else None,
                 C.c_void_p(tokens.data_ptr()), C.c_void_p(probs.data_ptr()),
                 C.c_void_p(ent.data_ptr()), C.c_void_p(wv.data_ptr()), C.c_void_p(atts.data_ptr()),
                 self._stream(), C.c_void_p(states.data_ptr()) if states is not None else None))
-        self._keep = (seq, lens, gt, u)   # alive until the stream has consumed them
+        self._keep = (seq, lens, gt, u, du)   # alive until the stream has consumed them
         self._recorded_N = N if record else None
         self.predicted_tokens, self.token_probs, self.neg_entropy = tokens, probs, ent
         self.word_vecs, self.atts = wv, atts
@@ -198,6 +216,31 @@ class AttentionSeq2Seq:
         return tokens, probs, ent, wv, atts
 
     __call__ = forward
+
+    def _dropout_uniforms(self, given, T, N):
+        """(enc, dec) device tensors for n2nmn_seq2seq_set_dropout; None = no dropout there."""
+        if given is None:
+            given = (None, None)
+        if not isinstance(given, (tuple, list)) or len(given) != 2:
+            raise ValueError('dropout_uniforms must be an (enc, dec) pair')
+        out = []
+        for side, flag, steps, g in (('encoder', self.encoder_dropout, T, given[0]),
+                                     ('decoder', self.decoder_dropout, self.T_decoder, given[1])):
+            shape = (steps, self.num_layers - 1, N, self.lstm_dim)
+            if g is not None and not flag:
+                raise ValueError('dropout uniforms given for the %s, whose dropout is off' % side)
+            if not flag or (g is None and self.num_layers == 1):   # one layer: nothing to drop
+                out.append(None)
+                continue
+            if g is None:
+                d = torch.rand(shape, dtype=torch.float32, device=self.device)
+            else:
+                d = g if isinstance(g, torch.Tensor) else torch.as_tensor(np.asarray(g, np.float32))
+                if tuple(d.shape) != shape:
+                    raise ValueError('%s dropout uniforms must be %s, got %s' % (side, shape, tuple(d.shape)))
+                d = d.to(self.device, torch.float32).contiguous()
+            out.append(d if self.num_layers > 1 else None)
+        return out
 
     def launch_count(self):
         return int(self._L.n2nmn_seq2seq_launch_count(self._h))

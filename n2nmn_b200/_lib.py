@@ -134,8 +134,6 @@ SIGNATURES = {
 
 
 def load():
-    global LIB_PATH
-    LIB_PATH = os.environ.get('N2NMN_LIB', LIB_PATH)   # experiment builds (build_variant) only
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             'n2nmn_b200: %s is missing. Build it with `python -m n2nmn_b200.build` (needs nvcc, '

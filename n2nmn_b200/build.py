@@ -26,19 +26,6 @@ def needs_build():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build_variant(name, defines):
-    """Experiment builds: lib/libn2nmn_b200_<name>.so with extra -D flags; selected at
-    run time with N2NMN_LIB=<path>. Never the default library."""
-    os.makedirs(LIBDIR, exist_ok=True)
-    out = os.path.join(LIBDIR, 'libn2nmn_b200_%s.so' % name)
-    cmd = [NVCC] + [f for f in FLAGS if f not in ('-Xptxas', '-v')] + ['-D' + d for d in defines] + \
-        [os.path.join(CSRC, s) for s in SOURCES] + ['-o', out]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError('nvcc failed:\n' + (r.stdout + r.stderr)[-4000:])
-    return out
-
-
 def build(force=False, verbose=False):
     if not force and not needs_build():
         return LIB

@@ -151,11 +151,8 @@ struct n2nmn_ctx {
   int node_smem_bytes = 0;
   int tree_smem_bytes = 0;
   int stack_cap = 0;           // attention-stack slots the tree kernel may use
-  int tree_cluster = 0;        // 0 = choose from the batch size; else forced (N2NMN_TREE_CLUSTER)
-  bool fp32_stencil = false;   // N2NMN_FP32_STENCIL=1: CUDA-core Transform stencil (A/B timing)
-  int text_ctas_per_group = 0; // 0 = one CTA per 64-column block
+  int tree_cluster = 0;        // 0 = choose from the batch size (n2nmn_set_tree_cluster)
   int proj_max_ctas = 0;       // 0 = one CTA per SM; else cap of the persistent projection grid
-  bool use_pdl = true;         // programmatic dependent launch between the three kernels
   n2nmn_sched module_sched;    // scratch schedule of n2nmn_module_fwd
   n2nmn_sched step_sched;      // scratch schedule of n2nmn_forward_tokens
   // training workspaces (allocated on first use; ready once every allocation and attribute is set)
@@ -361,9 +358,6 @@ auto wave_variant(int ks) { return ks == 5 ? &wave_kernel<5> : &wave_kernel<3>; 
 auto head_variant(int nn) {
   return nn == 16 ? &head_kernel<16> : nn == 8 ? &head_kernel<8> : &head_kernel<4>;
 }
-auto tail_gemm_variant(bool narrow) {
-  return narrow ? &head_tail_gemm_kernel<2> : &head_tail_gemm_kernel<4>;
-}
 // VQA walks Find-type nodes only (in two channel passes when wide); the conv families run the
 // Transform instantiation on a level with Transform nodes (tr) and the lighter one otherwise
 auto bwd_variant(bool vqa, bool tr, int ks, bool wide) {
@@ -404,7 +398,7 @@ int text_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, cudaStre
     const int qcols = quad_pitch(c->cfg.kernel_size) - quad_u_pitch(c->cfg.kernel_size);
     TRY(ctx_launch(c, quad_kernel,
                    dim3((unsigned)(1 + (qcols + kMmaCols - 1) / kMmaCols), (unsigned)((trn + 63) / 64)),
-                   kMmaThreads, mma_smem_bytes(4, kTextStages), st, {c->use_pdl}, c->md, c->tb,
+                   kMmaThreads, mma_smem_bytes(4, kTextStages), st, {true}, c->md, c->tb,
                    tr0, trn));
     prof_mark(c, "quad_kernel", st);
   }
@@ -417,7 +411,7 @@ int contraction_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, f
   if (S.work.empty()) return 0;
   ProjParams p;
   p.work = t.at<ProjWork>(t.o.work);
-  p.num_work = (int)S.work.size();
+  p.num_tiles = (int)S.work.size();
   p.total_rows = c->md.N * c->HW;
   p.num_seg = c->md.num_seg;
   p.seg_images = c->md.N;
@@ -439,38 +433,16 @@ int contraction_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, f
   p.mslot = t.at(t.o.mslot);
   p.num_images = (int)(S.mslot.size() / NUM_PROJ_SETS);
   p.mbuf = c->mbuf;
-  // persistent grid: CTA i walks the tiles i, i + CTAs, ... (two tiles per work item)
+  // persistent grid: CTA i walks the tiles i, i + CTAs, ...
   const int max_ctas = c->proj_max_ctas > 0 ? std::min(c->proj_max_ctas, c->num_sms) : c->num_sms;
-#if defined(N2NMN_EXP_PROJ_PAIRS)
-  // experiment build (proj_wgmma.cuh): an even grid of 2-CTA clusters, at most what fits at once
-  constexpr unsigned cluster = 2;
-  static int max_pairs = 0;
-  if (max_pairs == 0) {
-    cudaLaunchConfig_t oc;
-    std::memset(&oc, 0, sizeof(oc));
-    oc.gridDim = dim3((unsigned)(2 * (c->num_sms / 2)));
-    oc.blockDim = dim3(kProjThreads);
-    oc.dynamicSmemBytes = proj_smem_bytes();
-    cudaLaunchAttribute ca[1];
-    ca[0].id = cudaLaunchAttributeClusterDimension;
-    ca[0].val.clusterDim.x = 2; ca[0].val.clusterDim.y = 1; ca[0].val.clusterDim.z = 1;
-    oc.attrs = ca;
-    oc.numAttrs = 1;
-    CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, proj_wgmma_kernel, &oc));
-    if (max_pairs < 1) return fail(N2NMN_ERR_CUDA, "no 2-CTA cluster of the projection kernel fits");
-  }
-  const int ctas = 2 * std::max(1, std::min({p.num_work, max_ctas / 2, max_pairs}));
-#else
-  constexpr unsigned cluster = 1;
-  const int ctas = std::max(1, std::min(2 * p.num_work, max_ctas));
-#endif
+  const int ctas = std::max(1, std::min(p.num_tiles, max_ctas));
   if (c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) {
     const size_t smem = (size_t)(kSimtRows * kSimtKChunk + kSimtRows * c->Mp) * sizeof(float);
-    TRY(ctx_launch(c, proj_simt_kernel, 2 * p.num_work, 256, smem, st, {}, p));
+    TRY(ctx_launch(c, proj_simt_kernel, p.num_tiles, 256, smem, st, {}, p));
     prof_mark(c, "proj_simt_kernel", st);
   } else {
-    TRY(ctx_launch(c, proj_wgmma_kernel, ctas, kProjThreads, proj_smem_bytes(), st,
-                   {c->use_pdl, cluster}, c->tmaps, p));
+    TRY(ctx_launch(c, proj_wgmma_kernel, ctas, kProjThreads, proj_smem_bytes(), st, {true},
+                   c->tmaps, p));
     prof_mark(c, "proj_wgmma_kernel", st);
   }
   return 0;
@@ -506,9 +478,9 @@ int node_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, const No
       c->cfg.H, c->cfg.W, c->Mp, ks, c->cfg.map_dim, c->cfg.num_choices, slots,
       S.pooled_direct).total;
   const int wa = (write_arena ? kTreeWriteArena : 0) |
-                 (((c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) || c->fp32_stencil) ? kTreeFp32Stencil : 0);
+                 ((c->cfg.flags & N2NMN_FLAG_PROJ_FP32_SIMT) ? kTreeFp32Stencil : 0);
   TRY(ctx_launch(c, tree_variant(ks, S.pooled_direct), NQ * cs, kNodeThreads, smem, st,
-                 {c->use_pdl, (unsigned)cs}, nc, d_nodes, t.at(t.o.q_ptr), cs, slots, wa));
+                 {true, (unsigned)cs}, nc, d_nodes, t.at(t.o.q_ptr), cs, slots, wa));
   prof_mark(c, "tree_kernel", st);
   return 0;
 }
@@ -519,7 +491,7 @@ int head_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, const No
   if (!S.pooled_direct || S.head_work.empty()) return 0;
   if ((int)S.num_pool_rows > 2 * c->QB)
     return fail(N2NMN_ERR_CAPACITY, "too many pooled root nodes for this context");
-  const LaunchAttrs pdl{c->use_pdl};
+  const LaunchAttrs pdl{true};
   if (S.num_feat_rows > 0) {   // pooled features: one CTA per (root row, 128-channel chunk)
     const int HWp = (c->HW + 3) & ~3;
     const int quads = c->md.feat_pitch / 4;
@@ -535,7 +507,6 @@ int head_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, const No
   prof_mark(c, "head_kernel", st);
   if (!c->ehat) return 0;
   // fc_eltwise of the Describe-type roots as one GEMM per weight set
-  const bool tail_wgmma = c->ehat_lo && !std::getenv("N2NMN_TAIL_MMA_SYNC");
   for (int op : {OP_DESCRIBE, OP_SAME_PROPERTY}) {
     int r0 = 1 << 30, r1 = 0;
     for (const HeadWork& w : S.head_work)
@@ -543,24 +514,12 @@ int head_stage(n2nmn_ctx* c, const HostSchedule& S, const DevTables& t, const No
     if (r1 <= r0) continue;
     const int os = op == OP_DESCRIBE ? OS_DESCRIBE : OS_SAMEPROP;
     if (!c->out_wp[os]) return fail(N2NMN_ERR_STATE, "answer-head weights not packed");
-    if (tail_wgmma && c->out_wt_hi[os]) {
-      TRY(ctx_launch(c, head_tail_wgmma_kernel,
-                     dim3((unsigned)(c->Cpad / kHtN), (unsigned)((r1 - r0 + kHtM - 1) / kHtM)),
-                     kHtThreads, kHtSmemBytes, st, pdl, c->ht_maps[os], c->md.out_b[os],
-                     (float* const*)c->ehat_dst, r0, r1 - r0, (int)c->cfg.num_choices,
-                     (int)c->cfg.map_dim));
-    } else {
-      GemmOperands gp;
-      gp.a0 = c->ehat + (size_t)r0 * c->Mp; gp.k0 = c->cfg.map_dim; gp.lda0 = c->Mp;
-      gp.a1 = nullptr; gp.k1 = 0; gp.lda1 = 0;
-      gp.R = r1 - r0; gp.B = c->out_wp[os]; gp.ldb = c->Cp; gp.C = c->cfg.num_choices;
-      const bool narrow = gp.R <= 32;
-      TRY(ctx_launch(c, tail_gemm_variant(narrow),
-                     dim3((unsigned)((gp.C + kMmaCols - 1) / kMmaCols),
-                          (unsigned)(narrow ? (gp.R + 31) / 32 : (gp.R + 63) / 64)),
-                     kMmaThreads, mma_smem_bytes(narrow ? 2 : 4), st, pdl, gp, c->md.out_b[os],
-                     (float* const*)c->ehat_dst, r0));
-    }
+    TRY(ctx_launch(c, head_tail_wgmma_kernel,
+                   dim3((unsigned)(c->Cpad / kHtN), (unsigned)((r1 - r0 + kHtM - 1) / kHtM)),
+                   kHtThreads, kHtSmemBytes, st, pdl, c->ht_maps[os], c->md.out_b[os],
+                   (float* const*)c->ehat_dst, r0, r1 - r0, (int)c->cfg.num_choices,
+                   (int)c->cfg.map_dim));
+    // named after the retired mma.sync tail kernel: launch-time reports are keyed on this name
     prof_mark(c, "head_tail_gemm_kernel", st);
   }
   return 0;
@@ -799,8 +758,6 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
           TRY(encode_2d(c, &hm.b_lo, c->out_wt_lo[os], c->Mp, c->Cpad, c->Mp, kHtK, kHtN));
         }
     TRY(set_smem(head_tail_wgmma_kernel, (int)kHtSmemBytes));
-    for (bool narrow : {true, false})
-      TRY(set_smem(tail_gemm_variant(narrow), (int)mma_smem_bytes(narrow ? 2 : 4)));
   }
   c->head_nn = head_nodes_per_cta(c->Dk, c->Mp);
   c->head_smem_bytes = head_smem_layout(c->head_nn, c->Kp, c->Mp).total * (int)sizeof(float);
@@ -851,14 +808,6 @@ int n2nmn_create(const n2nmn_config* cfg, n2nmn_ctx** out) {
   c->module_sched.uid = g_uid++;
   c->module_sched.shp = c->shp;
   c->step_sched.shp = c->shp;
-  if (const char* e = std::getenv("N2NMN_NO_PDL")) c->use_pdl = (std::atoi(e) == 0);
-  if (const char* e = std::getenv("N2NMN_FP32_STENCIL")) c->fp32_stencil = (std::atoi(e) != 0);
-  if (const char* e = std::getenv("N2NMN_TEXT_CTAS")) c->text_ctas_per_group = std::max(0, std::atoi(e));
-  if (const char* e = std::getenv("N2NMN_PROJ_CTAS")) c->proj_max_ctas = std::max(0, std::atoi(e));
-  if (const char* e = std::getenv("N2NMN_TREE_CLUSTER")) {
-    const int v = std::atoi(e);
-    if (v == 1 || v == 2 || v == 4 || v == 8) c->tree_cluster = v;
-  }
   *out = owner.release();
   return 0;
 }
@@ -1537,7 +1486,7 @@ int bwd_walk(n2nmn_ctx* c, const BwdCtx& bc, const HostSchedule& S, const DevTab
     const int slices = n_tr > 0 ? std::max(3, std::min(kBwdSlicesMax, c->num_sms / n_tr))
                                 : std::max(2, std::min(6, 2 * c->num_sms / cnt));
     TRY(ctx_launch(c, bwd_variant(vqa, n_tr > 0, c->cfg.kernel_size, c->Mp > 512), dim3(cnt, slices),
-                   kNodeThreads, L.total * sizeof(float), st, {c->use_pdl}, bc,
+                   kNodeThreads, L.total * sizeof(float), st, {true}, bc,
                    t.at<NodeRec>(t.o.nodes), t.at(t.o.bwd_nodes), first, t.at(t.o.node_entry)));
   }
   prof_mark(c, "tree_bwd_kernel", st);
@@ -1764,12 +1713,6 @@ int n2nmn_set_grad_scale(n2nmn_ctx* c, float scale) {
   return 0;
 }
 
-#if defined(N2NMN_EXP_TIMELINE)
-extern "C" int n2nmn_exp_set_timeline(long long* dev_buf) {
-  return cudaMemcpyToSymbol(n2nmn::g_timeline, &dev_buf, sizeof(dev_buf)) == cudaSuccess ? 0 : -1;
-}
-#endif
-
 int n2nmn_set_tree_cluster(n2nmn_ctx* c, int ctas_per_question) {
   if (!c) return fail(N2NMN_ERR_ARG, "n2nmn_set_tree_cluster: null context");
   const int v = ctas_per_question;
@@ -1789,8 +1732,7 @@ int n2nmn_set_proj_ctas(n2nmn_ctx* c, int max_ctas) {
 int n2nmn_set_text_ctas_per_group(n2nmn_ctx* c, int n) {
   if (!c) return fail(N2NMN_ERR_ARG, "n2nmn_set_text_ctas_per_group: null context");
   if (n < 0) return fail(N2NMN_ERR_ARG, "n2nmn_set_text_ctas_per_group: n must be >= 0");
-  c->text_ctas_per_group = n;
-  return 0;
+  return 0;   // retired: the text kernel's grid follows the schedule (see the header)
 }
 
 int n2nmn_set_profiling(n2nmn_ctx* c, int enabled) {

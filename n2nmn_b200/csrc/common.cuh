@@ -11,10 +11,7 @@ constexpr int kMaxProjNodesPerPass = 8;
 // One launch may cover several independent batches ("segments": separate feature / word-vector /
 // score buffers of identical shape) so that the kernels see enough work per launch. Images and
 // questions are numbered across the segments: g = seg * N + b.
-#ifndef N2NMN_MAX_SEG
-#define N2NMN_MAX_SEG 16
-#endif
-constexpr int kMaxSeg = N2NMN_MAX_SEG;
+constexpr int kMaxSeg = 16;
 
 // Opcodes mirror enum n2nmn_op in include/n2nmn_b200.h.
 enum Op : int {
@@ -111,11 +108,10 @@ __host__ __device__ inline int quad_pitch(int ksize) { return (quad_rows(ksize) 
 // Host-compiled launch tables (built by schedule.cpp, consumed by the kernels).
 struct TextGroup { int32_t set, start, count, pad; };   // <= kTextRowsPerCta rows of one text set
 constexpr int kTextRowsPerCta = 64;
-// One work item of the contraction kernel = a PAIR of 128-row tiles of the same weight set (the
-// tiles share nothing but the weight matrix, so they may come from different images, passes or
-// segments). row0 = first row inside the segment's [N*HW] row axis; pass = which block of <= 8
-// Find consumers the fused epilogue serves, or -1 for a filler tile (odd tile count: skipped).
-struct ProjWork { int32_t row0[2], seg[2], pass[2], set, pad; };
+// One tile of the contraction kernel: 128 rows of one segment against one weight set. row0 = first
+// row inside the segment's [N*HW] row axis; pass = which block of <= 8 Find consumers the fused
+// epilogue serves.
+struct ProjWork { int32_t row0, seg, pass, set; };
 // One CTA of the answer-head kernel (head_kernel.cuh): `count` <= kHeadNodesMax root nodes of
 // the same type (Describe or SameProperty), listed in head_list[first .. first+count).
 struct HeadWork { int32_t first, count, op, pad; };
@@ -142,23 +138,6 @@ __device__ __forceinline__ void pdl_trigger() {
 __device__ __forceinline__ void pdl_wait() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
 }
-
-// Timeline instrumentation (experiment builds only, -DN2NMN_EXP_TIMELINE): clock64 stamps per CTA.
-#if defined(N2NMN_EXP_TIMELINE)
-__device__ long long* g_timeline = nullptr;   // [kernel 0..2][cta < 512][64]: clock64 | globaltimer
-#define N2NMN_STAMP(kernel, slot)                                                          \
-  do {                                                                                     \
-    const int cta_ = blockIdx.y * gridDim.x + blockIdx.x;                                  \
-    if (g_timeline && cta_ < 512 && (slot) < 32 && (threadIdx.x & 31) == 0) {              \
-      unsigned long long gt_;                                                              \
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_));                              \
-      g_timeline[((kernel) * 512 + cta_) * 64 + (slot)] = clock64();                       \
-      g_timeline[((kernel) * 512 + cta_) * 64 + 32 + (slot)] = (long long)gt_;             \
-    }                                                                                      \
-  } while (0)
-#else
-#define N2NMN_STAMP(kernel, slot) do {} while (0)
-#endif
 
 // word_vecs row of (time t, global image g): segment g / N, row t*N + (g % N)
 __device__ __forceinline__ const float* word_vec_row(const DevModel& md, int t, int g) {

@@ -20,7 +20,6 @@
 // fp32 here is tighter than the TF32 maps it replaces.
 #pragma once
 #include "node_eval.cuh"
-#include "mma_tile.cuh"
 
 namespace n2nmn {
 
@@ -373,37 +372,6 @@ head_kernel(const NodeCtx c, const NodeRec* __restrict__ nodes,
       for (int n = 0; n < NN; ++n)
         if (n < cnt) s_outp[n][cl] = acc[n] + b;
     }
-  }
-}
-
-// scores[root] = ê[root]·W + b for the roots [row0, row0 + p.R) of the head list: fc_eltwise of the
-// Describe-type heads when the class count is large (models_vqa/nmn3_modules.py:236-240: 3001
-// answers). One fp32-parity tile GEMM (mma_tile.cuh) over all roots of the launch instead of every
-// head CTA streaming the whole [M][C] matrix (12 MB at VQA) for its 4-8 roots, which was 55 % of
-// the VQA D=514 step. p.a0 = ê rows, p.B = the weight matrix with rows pitched to a multiple of 4.
-// grid = (ceil(C/32), ceil(R/(16 WM)))
-template <int WM>
-__global__ void __launch_bounds__(kMmaThreads)
-head_tail_gemm_kernel(GemmOperands p, const float* __restrict__ bias, float* const* __restrict__ dst,
-                      int row0) {
-  pdl_trigger();
-  extern __shared__ __align__(16) float mma_smem[];
-  const int r0 = blockIdx.y * 16 * WM, c0 = blockIdx.x * kMmaCols;
-  float acc[4][4];
-  if (!mma_tile<WM>(mma_smem, p, r0, c0, acc, [] {})) return;
-  const int lane = threadIdx.x & 31, wm = (threadIdx.x >> 5) % WM, g = lane >> 2, tig = lane & 3;
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    const int r = r0 + wm * 16 + g + 8 * hh;
-    if (r >= p.R) continue;
-    float* out = dst[row0 + r];
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int cc = c0 + nt * 8 + 2 * tig + j;
-        if (cc < p.C) out[cc] = acc[nt][hh * 2 + j] + bias[cc];
-      }
   }
 }
 

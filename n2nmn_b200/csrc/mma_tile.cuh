@@ -1,6 +1,6 @@
 // 64 x 32 (or 32 x 32) fp32-parity GEMM tile on mma.sync m16n8k8 with error-compensated TF32,
 // operands streamed through a cp.async ring. Shared by the seq2seq kernels (seq2seq.cu) and the
-// large-class-count answer head (head_kernel.cuh).
+// text projections (text_proj.cuh).
 #pragma once
 #include "common.cuh"
 #include "tile_gemm.cuh"
@@ -21,16 +21,14 @@ namespace n2nmn {
 constexpr int kMmaCols = 32, kMmaKC = 128, kMmaThreads = 256;
 constexpr int kMmaAPitch = kMmaKC + 4;     // rows g / g+8 and k / k+4 of a fragment: distinct banks
 constexpr int kMmaBPitch = kMmaCols + 8;
-#ifndef N2NMN_S2S_STAGES_NARROW
-#define N2NMN_S2S_STAGES_NARROW 5
-#endif
 // a stage = A [16 WM][kMmaAPitch] then B [kMmaKC][kMmaBPitch]: 3 stages (162 KB) for 64-row tiles,
 // 5 stages (187 KB) for 32-row tiles: at N <= 64 a step is bound by the latency of its operand
 // stream, i.e. by the bytes in flight per SM (measured 2.59 -> 1.97 ms per batch from 3 to 5)
 __host__ __device__ constexpr int mma_stage_floats(int wm) {
   return 16 * wm * kMmaAPitch + kMmaKC * kMmaBPitch;
 }
-__host__ __device__ constexpr int mma_stages(int wm) { return wm == 2 ? N2NMN_S2S_STAGES_NARROW : 3; }
+constexpr int kMmaStagesNarrow = 5;
+__host__ __device__ constexpr int mma_stages(int wm) { return wm == 2 ? kMmaStagesNarrow : 3; }
 __host__ __device__ constexpr size_t mma_smem_bytes(int wm, int stages = 0) {
   return (size_t)(stages > 0 ? stages : mma_stages(wm)) * mma_stage_floats(wm) * sizeof(float);
 }

@@ -35,7 +35,7 @@ struct NodeCtx {
   float* phi_out;
   // answer heads with many classes (VQA: 3001): head_kernel leaves the normalised vector ê of
   // root r (its position in the head list) in ehat[r][Mp] and the address of its score row in
-  // ehat_dst[r]; head_tail_gemm_kernel does the fc_eltwise product as one GEMM (nullptr otherwise)
+  // ehat_dst[r]; head_tail_wgmma_kernel does the fc_eltwise product as one GEMM (nullptr otherwise)
   float* ehat;
   float* ehat_lo;      // ê - trunc_tf32(ê) for the wgmma tail (head_tail_wgmma.cuh), or nullptr
   float** ehat_dst;

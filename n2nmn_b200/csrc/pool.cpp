@@ -11,7 +11,7 @@
 // queued it runs one. There is no reference counterpart: the reference's executor is a Python loop
 // around session.run (exp_clevr/eval_clevr.py:96-133), one batch at a time.
 //
-// Uses nothing but the public C ABI of include/n2nmn_b200.h.
+// Uses nothing but the public C ABI of include/n2nmn_b200.h (and the segment limit of common.cuh).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "../../include/n2nmn_b200.h"
+#include "common.cuh"
 
 namespace {
 
@@ -55,10 +56,7 @@ struct Worker {
 // step is ~10 us of host work, a futex wake-up is 50-100 us, so a sleeping worker turns a short
 // burst of submissions (the driver's --steps 20) into a measurement of wake-up latency.
 constexpr int kSpinMicros = 300;
-#ifndef N2NMN_MAX_SEG
-#define N2NMN_MAX_SEG 16
-#endif
-constexpr int kMaxGroup = N2NMN_MAX_SEG;   // = kMaxSeg of the kernels (common.cuh)
+constexpr int kMaxGroup = n2nmn::kMaxSeg;   // batches one set of launches may cover
 
 inline void cpu_relax() {
 #if defined(__x86_64__) || defined(__i386__)

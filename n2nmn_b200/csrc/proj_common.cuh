@@ -17,8 +17,8 @@
 namespace n2nmn {
 
 struct ProjParams {
-  const ProjWork* work;   // pair items (two 128-row tiles each, common.cuh)
-  int num_work;
+  const ProjWork* work;   // 128-row tiles (common.cuh)
+  int num_tiles;
   int total_rows;   // rows of ONE segment: N*HW
   int num_seg;      // segments covered by this launch
   int seg_images;   // N: images per segment (global image g = seg*N + b)

@@ -20,14 +20,11 @@ proj_simt_kernel(ProjParams p) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int col_iters = p.Mp / 256;
 
-  // one CTA per TILE: CTA 2i / 2i+1 take the two halves of pair item i
-  for (int ti = blockIdx.x; ti < 2 * p.num_work; ti += gridDim.x) {
-    const ProjWork wk = p.work[ti >> 1];
-    const int hf = ti & 1;
-    const int wk_pass = wk.pass[hf], wk_row0 = wk.row0[hf];
-    if (wk_pass < 0) continue;   // filler half of an odd pair
-    const int g0 = wk.seg[hf] * p.seg_images;
-    const float* __restrict__ feat = p.feat_seg[wk.seg[hf]];
+  for (int ti = blockIdx.x; ti < p.num_tiles; ti += gridDim.x) {   // one CTA per tile
+    const ProjWork wk = p.work[ti];
+    const int wk_pass = wk.pass, wk_row0 = wk.row0;
+    const int g0 = wk.seg * p.seg_images;
+    const float* __restrict__ feat = p.feat_seg[wk.seg];
     const float* __restrict__ W = p.w_orig[wk.set];
     for (int r0 = 0; r0 < 128; r0 += kSimtRows) {
       const int row_base = wk_row0 + r0;

@@ -3,12 +3,11 @@
 // what is fused.
 //
 // Tiling. One tile = 128 rows of the flattened (image, pixel) axis x all Mp output columns, walked
-// as Mp/256 N-tiles. A work item (common.cuh) holds two tiles; the persistent grid walks the tiles
-// t = blockIdx.x, blockIdx.x + gridDim.x, ... of item t/2, half t%2. Filler tiles (pass < 0) are
-// skipped by every role. K is streamed in 32-float (128-byte, one swizzle atom) slices through a
-// 4-stage TMA ring (SWIZZLE_128B, K-major): per stage the 128 feature rows (16 KB) and the 256
-// weight columns of the N-tile (32 KB). fp32 operands are read as TF32 straight from the caller's
-// fp32 feature grid: no conversion pass.
+// as Mp/256 N-tiles. The persistent grid walks the schedule's tile list (common.cuh): CTA i takes
+// the tiles i, i + gridDim.x, ... K is streamed in 32-float (128-byte, one swizzle atom) slices
+// through a 4-stage TMA ring (SWIZZLE_128B, K-major): per stage the 128 feature rows (16 KB) and
+// the 256 weight columns of the N-tile (32 KB). fp32 operands are read as TF32 straight from the
+// caller's fp32 feature grid: no conversion pass.
 //
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one elected lane; its registers are handed
 // to the consumers with setmaxnreg), warpgroups 1 and 2 = consumers. Consumer warpgroup w owns rows
@@ -51,31 +50,6 @@ struct ProjTensorMaps {
   CUtensorMap b[NUM_PROJ_SETS];      // W^T [Mp, Kp] fp32 (K-major), box 32 x 128 (half an N-tile)
 };
 
-// Experiment builds (tools/build_variants.py attrib; never the default library) that remove one
-// part of the kernel's work to attribute its time. Their outputs are wrong by design.
-//   N2NMN_EXP_PROJ_NO_EPI  consumers skip the epilogue (bias, stored maps, Find consumers)
-//   N2NMN_EXP_PROJ_NO_STORE  the epilogue writes no stored maps
-//   N2NMN_EXP_PROJ_NO_FIND   the epilogue skips the fused Find consumers
-//   N2NMN_EXP_PROJ_NO_B    the producer streams only the feature box; the MMA reads stale weights
-//   N2NMN_EXP_PROJ_NO_MMA  consumers wait for and release every stage without issuing wgmma
-//   N2NMN_EXP_PROJ_PAIRS   (results stay exact) the grid runs as 2-CTA clusters: CTA r of a
-//                          cluster takes half r of every work item it visits (blockIdx.x =
-//                          2 * cluster + r keeps the tile walk below), fetches weight box r (128
-//                          of the 256 columns) and multicasts it into both CTAs' stage, so each
-//                          CTA pulls 32 KB per stage from L2 instead of 48 KB. A stage is refilled
-//                          once the consumers of both CTAs have released it (16 arrivals), and a
-//                          filler half runs the ring and the MMA for its partner, writing nothing.
-#if defined(N2NMN_EXP_PROJ_PAIRS)
-constexpr bool kPair = true;
-#else
-constexpr bool kPair = false;
-#endif
-#if defined(N2NMN_EXP_PROJ_NO_B)
-constexpr int kStageTxBytes = kABytes;
-#else
-constexpr int kStageTxBytes = kStageBytes;
-#endif
-
 __global__ void __launch_bounds__(kProjThreads, 1)
 proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p) {
   extern __shared__ __align__(1024) uint8_t proj_smem_raw[];
@@ -87,8 +61,6 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;   // 0 = producer, 1..2 = consumers
-  const int n_tiles_total = 2 * p.num_work;
-  const uint32_t rank = kPair ? ptx::cluster_ctarank() : 0u;
   pdl_trigger();   // let the node kernel's CTAs start prefetching their parameters
 
   if (threadIdx.x == 0) {
@@ -97,12 +69,11 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
     for (int i = 0; i < NUM_PROJ_SETS; ++i) ptx::prefetch_tensormap(&tm.b[i]);
     for (int s = 0; s < kProjStages; ++s) {
       ptx::mbar_init(&full[s], 1);   // the producer's arrive.expect_tx
-      ptx::mbar_init(&empty[s], kPair ? 16 : 8);  // one arrive per consumer warp (of both CTAs)
+      ptx::mbar_init(&empty[s], 8);  // one arrive per consumer warp
     }
     ptx::fence_barrier_init();
   }
-  if (kPair) ptx::cluster_sync();   // the partner must see the barriers initialised
-  else __syncthreads();
+  __syncthreads();
 
   if (wg == 0) {
     // ===================================================================== TMA producer
@@ -110,35 +81,23 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
     if (warp == 0 && ptx::elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int ti = blockIdx.x; ti < n_tiles_total; ti += gridDim.x) {
-        const ProjWork* wk = p.work + (ti >> 1);
-        const int hf = ti & 1;
-        if (!kPair && wk->pass[hf] < 0) continue;
-        const int row0 = wk->row0[hf], seg = wk->seg[hf], set = wk->set;
+      for (int ti = blockIdx.x; ti < p.num_tiles; ti += gridDim.x) {
+        const ProjWork* wk = p.work + ti;
+        const int row0 = wk->row0, seg = wk->seg, set = wk->set;
         for (int nt = 0; nt < p.n_tiles; ++nt) {
           for (int kb = 0; kb < p.k_blocks; ++kb) {
             ptx::mbar_wait(&empty[stage], phase ^ 1);
-            ptx::mbar_arrive_expect_tx(&full[stage], kStageTxBytes);
+            ptx::mbar_arrive_expect_tx(&full[stage], kStageBytes);
             uint8_t* dst = smem + stage * kStageBytes;
             ptx::tma_load_2d(dst, &tm.a[seg], kb * kBK, row0, &full[stage]);
-#if !defined(N2NMN_EXP_PROJ_NO_B)
-            if (kPair) {
-              ptx::tma_load_2d_multicast(dst + kABytes + rank * (kBNHalf * kBK * 4), &tm.b[set],
-                                         kb * kBK, nt * kBN + rank * kBNHalf, &full[stage], 0x3);
-            } else {
-              ptx::tma_load_2d(dst + kABytes, &tm.b[set], kb * kBK, nt * kBN, &full[stage]);
-              ptx::tma_load_2d(dst + kABytes + kBNHalf * kBK * 4, &tm.b[set], kb * kBK,
-                               nt * kBN + kBNHalf, &full[stage]);
-            }
-#endif
+            ptx::tma_load_2d(dst + kABytes, &tm.b[set], kb * kBK, nt * kBN, &full[stage]);
+            ptx::tma_load_2d(dst + kABytes + kBNHalf * kBK * 4, &tm.b[set], kb * kBK,
+                             nt * kBN + kBNHalf, &full[stage]);
             if (++stage == kProjStages) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
-    // no CTA of a pair leaves while its partner may still write into its ring or arrive on its
-    // barriers
-    if (kPair) ptx::cluster_sync();
     return;
   }
 
@@ -150,33 +109,24 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
   // tauw / tau2 come from the text-projection kernel, which may still be running (PDL); the
   // producer never touches its output and starts immediately.
   pdl_wait();
-  auto release = [&](int s) {   // one arrive per consumer warp (and on the partner's barrier)
-    if (lane == 0) {
-      ptx::mbar_arrive(&empty[s]);
-      if (kPair) ptx::mbar_arrive_cluster(&empty[s], rank ^ 1u);
-    }
+  auto release = [&](int s) {   // one arrive per consumer warp
+    if (lane == 0) ptx::mbar_arrive(&empty[s]);
   };
   int stage = 0;
   uint32_t phase = 0;
   float acc[kBN / 2];
-#if defined(N2NMN_EXP_PROJ_NO_MMA)
-#pragma unroll
-  for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
-#endif
-  for (int ti = blockIdx.x; ti < n_tiles_total; ti += gridDim.x) {
-    const ProjWork* wkp = p.work + (ti >> 1);
-    const int hf = ti & 1;
-    const int pass = wkp->pass[hf];
-    if (!kPair && pass < 0) continue;
-    const int row0 = wkp->row0[hf], set = wkp->set;
-    const int g0 = wkp->seg[hf] * p.seg_images;   // first image of this tile's segment
+  for (int ti = blockIdx.x; ti < p.num_tiles; ti += gridDim.x) {
+    const ProjWork* wkp = p.work + ti;
+    const int pass = wkp->pass;
+    const int row0 = wkp->row0, set = wkp->set;
+    const int g0 = wkp->seg * p.seg_images;   // first image of this tile's segment
     // the two rows of this thread and their consumers
     int e_beg[2], n_nodes[2], pix[2];
     float* mdst[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = row0 + rbase + 8 * h;
-      const bool row_ok = pass >= 0 && row < p.total_rows;   // (a filler half has none)
+      const bool row_ok = row < p.total_rows;
       const int b = row_ok ? row / p.HW : 0;
       pix[h] = row - b * p.HW;
       e_beg[h] = 0;
@@ -198,9 +148,6 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
       // ---- mainloop: 4 wgmma per stage; a stage is released once the next one's are issued
       for (int kb = 0; kb < p.k_blocks; ++kb) {
         ptx::mbar_wait(&full[stage], phase);
-#if defined(N2NMN_EXP_PROJ_NO_MMA)
-        release(stage);
-#else
         const uint32_t sa = ptx::smem_u32(smem + stage * kStageBytes);
         const uint64_t da = ptx::make_smem_desc_sw128(sa + (wg - 1) * 64 * 128);
         const uint64_t db = ptx::make_smem_desc_sw128(sa + kABytes);
@@ -210,7 +157,6 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
         for (int k = 0; k < kBK / kWgmmaK; ++k)   // 32 bytes (2 x 16-byte units) along K
           ptx::wgmma_m64n256k8_tf32(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
         ptx::wgmma_commit();
-#if !defined(N2NMN_EXP_PROJ_NO_EPI) && !defined(N2NMN_EXP_PROJ_NO_FIND)
         if (kb == 0 && set == PS_FIND) {
           // While the first slice's MMAs run: pull the text rows the epilogue reads (this N-tile's
           // columns of tauw / tau2 for every consumer node of the thread's two rows, 8 lines per
@@ -231,21 +177,14 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
             }
           }
         }
-#endif
         ptx::wgmma_wait<1>();
         ptx::fence_regs(acc);
         if (kb > 0) release(stage == 0 ? kProjStages - 1 : stage - 1);
-#endif
         if (++stage == kProjStages) { stage = 0; phase ^= 1; }
       }
-#if !defined(N2NMN_EXP_PROJ_NO_MMA)
       ptx::wgmma_wait<0>();
       ptx::fence_regs(acc);
       release(stage == 0 ? kProjStages - 1 : stage - 1);
-#endif
-#if defined(N2NMN_EXP_PROJ_NO_EPI)
-      continue;
-#endif
 
       // ---- epilogue on the accumulator: + bias, stored map, fused Find consumers
       const int colq = nt * kBN + 2 * q;   // + 8 j: columns of registers 4j .. 4j+3
@@ -255,7 +194,6 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
         acc[4 * j + 0] += bb.x; acc[4 * j + 1] += bb.y;
         acc[4 * j + 2] += bb.x; acc[4 * j + 3] += bb.y;
       }
-#if !defined(N2NMN_EXP_PROJ_NO_STORE)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (mdst[h] != nullptr) {
@@ -265,10 +203,6 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
                 make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
       }
-#endif
-#if defined(N2NMN_EXP_PROJ_NO_FIND)
-      continue;
-#endif
       if (set != PS_FIND) continue;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -320,7 +254,6 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
       }
     }
     // the N-tiles of a row meet here (the same thread wrote every partial sum it reads)
-#if !defined(N2NMN_EXP_PROJ_NO_EPI) && !defined(N2NMN_EXP_PROJ_NO_FIND)
     if (set == PS_FIND && q == 0) {
       const float b2 = __ldg(p.elt_b);
 #pragma unroll
@@ -332,9 +265,7 @@ proj_wgmma_kernel(const __grid_constant__ ProjTensorMaps tm, const ProjParams p)
         }
       }
     }
-#endif
   }
-  if (kPair) ptx::cluster_sync();
 }
 
 }  // namespace n2nmn

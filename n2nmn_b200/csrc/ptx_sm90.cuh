@@ -69,38 +69,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
         "r"(smem_u32(bar))
       : "memory");
 }
-// The same tile delivered to the same shared-memory offset in every CTA of `cta_mask`; each
-// destination CTA's mbarrier at `bar`'s offset receives complete_tx for the box's bytes.
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* map, int c0,
-                                                      int c1, uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      ".multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1),
-        "r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-
-// ---- clusters -------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// Every thread of every CTA of the cluster meets here; release / acquire order the shared-memory
-// (and mbarrier) operations before it against those after it, cluster-wide.
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
-}
-// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster; release at
-// cluster scope orders this thread's earlier reads of the stage before the remote producer's refill.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}\n"
-      ::"r"(smem_u32(bar)), "r"(cta) : "memory");
-}
 
 // ---- wgmma ----------------------------------------------------------------------------------
 // Shared-memory matrix descriptor for a K-major tile whose rows are 128 bytes (32 fp32) wide and

@@ -249,25 +249,10 @@ int finalize_schedule(const SchedShape& shp, int images_per_seg, HostSchedule* o
   // Tiles (128 rows of one segment x one layer x one pass of <= 8 Find consumers) in tile-major
   // order: the layers that need the same 128 rows of features are handed out at about the same
   // time, so the A tile is fetched from HBM once and the other layers hit it in L2 (matters once
-  // the batch no longer fits in L2). Two tiles of the SAME layer form one work item; the default
-  // kernel's persistent CTAs walk single tiles, and the pairing lets a 2-CTA cluster share the
-  // weight slices (the N2NMN_EXP_PROJ_PAIRS build of proj_wgmma.cuh). The two tiles share only
-  // the weight matrix, so a tile is paired with the next tile of its layer wherever that one comes
-  // from. A layer with an odd tile count gets a filler half (pass = -1: skipped by the single-CTA
-  // kernel; the cluster form runs the MMA on the repeated tile and writes nothing).
+  // the batch no longer fits in L2).
   const int seg_rows = images_per_seg * HW;
   const int tiles_per_seg = (seg_rows + 127) / 128;
   S.work.reserve((size_t)tiles_per_seg * std::max(1, S.num_seg));
-  struct Half { int row0, seg, pass; bool open; };
-  Half pending[NUM_PROJ_SETS];
-  for (int set = 0; set < NUM_PROJ_SETS; ++set) pending[set].open = false;
-  auto emit = [&](int set, const Half& a, const Half& b) {
-    ProjWork w;
-    w.row0[0] = a.row0; w.seg[0] = a.seg; w.pass[0] = a.pass;
-    w.row0[1] = b.row0; w.seg[1] = b.seg; w.pass[1] = b.pass;
-    w.set = set; w.pad = 0;
-    S.work.push_back(w);
-  };
   for (int seg = 0; seg < std::max(1, S.num_seg); ++seg) {
     const int g0 = seg * images_per_seg;
     for (int tile = 0; tile < tiles_per_seg; ++tile) {
@@ -281,20 +266,10 @@ int finalize_schedule(const SchedShape& shp, int images_per_seg, HostSchedule* o
       }
       for (int set = 0; set < NUM_PROJ_SETS; ++set) {
         const int passes = (need[set] + kMaxProjNodesPerPass - 1) / kMaxProjNodesPerPass;
-        for (int pass = 0; pass < passes; ++pass) {
-          const Half h{r0, seg, pass, true};
-          if (pending[set].open) { emit(set, pending[set], h); pending[set].open = false; }
-          else pending[set] = h;
-        }
+        for (int pass = 0; pass < passes; ++pass) S.work.push_back(ProjWork{r0, seg, pass, set});
       }
     }
   }
-  for (int set = 0; set < NUM_PROJ_SETS; ++set)
-    if (pending[set].open) {
-      Half filler = pending[set];
-      filler.pass = -1;
-      emit(set, pending[set], filler);
-    }
 
   // ---- shared-memory stack slots for the tree kernel: a map lives from its producer to its
   //      (single) consumer; inputs are released before the output is placed, so in-place reuse

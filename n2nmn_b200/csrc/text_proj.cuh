@@ -36,7 +36,6 @@ __global__ void __launch_bounds__(kMmaThreads)
 text_proj_kernel(DevModel md, TextBufs tb, TextSetRows rows,
                  const int32_t* __restrict__ text_t, const int32_t* __restrict__ text_b) {
   pdl_trigger();   // the contraction kernel only needs our output in its epilogue
-  if (threadIdx.x == 0) N2NMN_STAMP(0, 0);
   const int M = md.M, Mp = md.Mp;
   TextGroup g;   // blockIdx.y-th group, groups never straddle weight sets
   {
@@ -64,7 +63,6 @@ text_proj_kernel(DevModel md, TextBufs tb, TextSetRows rows,
   extern __shared__ __align__(16) float mma_smem[];
   float acc[4][4];
   if (!mma_tile<4, true, kTextStages>(mma_smem, op, 0, c0, acc, [] {})) return;
-  if (threadIdx.x == 0) N2NMN_STAMP(0, 4);
   const int lane = threadIdx.x & 31, wm = (threadIdx.x >> 5) & 3, gq = lane >> 2, tig = lane & 3;
 #pragma unroll
   for (int nt = 0; nt < 4; ++nt) {
@@ -88,7 +86,6 @@ text_proj_kernel(DevModel md, TextBufs tb, TextSetRows rows,
       *reinterpret_cast<float2*>(tb.tau2 + idx) = make_float2(t0 * t0, t1 * t1);
     }
   }
-  if (threadIdx.x == 0) N2NMN_STAMP(0, 5);
 }
 
 // (u, Q) of the Transform nodes (common.cuh): tq[row, o] = Σ_c (o < n ? tau : tau²)[row, c] ·

@@ -178,7 +178,6 @@ tree_kernel(const NodeCtx c, const NodeRec* __restrict__ nodes, const int32_t* _
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int gwarp = co.rank * nwarps + warp, gwarps = co.size * nwarps;
 
-  if (threadIdx.x == 0) N2NMN_STAMP(2, 0);
   // ---- prologue part 1: launch tables and weights only (overlaps the predecessors)
   const float* head_w = nullptr;
   const bool nodes_in_smem = (end - beg) <= kTreeNodeCap;
@@ -207,14 +206,12 @@ tree_kernel(const NodeCtx c, const NodeRec* __restrict__ nodes, const int32_t* _
     }
   }
   // ---- the attention arena, stored maps and text projections come from the preceding kernels
-  if (threadIdx.x == 0) N2NMN_STAMP(2, 1);
   pdl_wait();
   // the node records staged above are read by every thread below. (A CTA of the first wave sits in
   // pdl_wait long enough for the writes to land; a CTA that starts after the predecessor has
   // finished does not — without this barrier the questions of the second wave read stale records:
   // tools/dbg_group.py, r2.)
   __syncthreads();
-  if (threadIdx.x == 0) N2NMN_STAMP(2, 2);
   if (beg == end) {   // invalid layout: zeros(num_choices) (models_clevr/nmn3_model.py:144-155)
     if (co.rank == 0)
       for (int i = threadIdx.x; i < md.C; i += blockDim.x) score_row(c, q)[i] = 0.f;
@@ -250,7 +247,6 @@ tree_kernel(const NodeCtx c, const NodeRec* __restrict__ nodes, const int32_t* _
     __syncthreads();
   }
 
-  if (threadIdx.x == 0) N2NMN_STAMP(2, 3);
   int exch = 0;        // cluster exchanges so far: selects the double-buffered outbuf / part half
   int nfilter = 0, ntext = 0, nquad = 0;
   for (int i = beg; i < end; ++i) {
@@ -327,7 +323,6 @@ tree_kernel(const NodeCtx c, const NodeRec* __restrict__ nodes, const int32_t* _
           out[p] = (nd.op == OP_AND) ? fminf(in0[p], in1[p]) : fmaxf(in0[p], in1[p]);
         break;
       case OP_TRANSFORM: {
-        if (threadIdx.x == 0) N2NMN_STAMP(2, 20);
         // TransformModule, conv variant (models_clevr/nmn3_modules.py:185-216, SHAPES :71-101),
         // as the quadratic form of common.cuh; every CTA of a cluster computes the whole map
         if (KS > 1) {
@@ -350,9 +345,7 @@ tree_kernel(const NodeCtx c, const NodeRec* __restrict__ nodes, const int32_t* _
             s.pad[(y + R) * PW + x + R] = in0[p];
           }
           __syncthreads();
-          if (threadIdx.x == 0) N2NMN_STAMP(2, 21);
           transform_quad<KS>(s.pad, qc, md.elt_b[ES_TRANSFORM][0], out, Hh, Ww);
-          if (threadIdx.x == 0) N2NMN_STAMP(2, 22);
         }
         break;
       }
@@ -505,7 +498,6 @@ tree_kernel(const NodeCtx c, const NodeRec* __restrict__ nodes, const int32_t* _
       }
     }
     __syncthreads();   // this node's stack writes are visible to the CTA's next node
-    if (threadIdx.x == 0) N2NMN_STAMP(2, 4 + (i - beg));
     if (write_arena && co.rank == 0 && out != nullptr && nd.op != OP_FIND) {
       float* g = c.arena + (size_t)nd.out * HW;
       for (int p = threadIdx.x; p < HW; p += blockDim.x) g[p] = out[p];

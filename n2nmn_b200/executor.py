@@ -14,8 +14,6 @@ compiled batch (n2nmn_run_schedule). Rows of invalid layouts are zeros
 """
 from __future__ import annotations
 
-import os
-
 import ctypes as C
 
 import numpy as np
@@ -307,8 +305,6 @@ class ExecutorPool:
         if max_group is None:   # ~1024 questions per launch set: the contraction kernel's CTAs
             # then walk 10+ tiles each (0.49 of the TF32 peak against 0.42 at 512; 6.2 M vs 5.3 M q/s)
             max_group = 1 if num_streams == 1 else max(1, min(16, 1024 // max(nb, 1)))
-        if 'N2NMN_MAX_GROUP' in os.environ:
-            max_group = int(os.environ['N2NMN_MAX_GROUP'])
         self.max_group = int(max_group)
         first = LayoutExecutor(family, image_feat_grid, word_vecs, num_choices, assembler,
                                weights=weights, max_group=self.max_group, **ctx_kwargs)
@@ -326,19 +322,13 @@ class ExecutorPool:
             tree_cluster = 0 if num_streams == 1 else 1
         if proj_ctas is None:
             proj_ctas = 0
-        text_ctas = 0 if num_streams == 1 else 1
-        if 'N2NMN_TREE_CLUSTER' in os.environ:
-            tree_cluster = int(os.environ['N2NMN_TREE_CLUSTER'])
-        if 'N2NMN_PROJ_CTAS' in os.environ:
-            proj_ctas = int(os.environ['N2NMN_PROJ_CTAS'])
         self.tree_cluster, self.proj_ctas = tree_cluster, proj_ctas
-        if 'N2NMN_TEXT_CTAS' in os.environ:
-            text_ctas = int(os.environ['N2NMN_TEXT_CTAS'])
-        self.text_ctas_per_group = text_ctas
+        # retired knob of the round-1 text kernel (n2nmn_set_text_ctas_per_group is a no-op): the
+        # value the pool used to pass is kept readable for callers of the ABI-2 Python API
+        self.text_ctas_per_group = 0 if num_streams == 1 else 1
         for ex in self.executors:
             ex.set_tree_cluster(tree_cluster)
             ex.set_proj_ctas(proj_ctas)
-            ex.set_text_ctas_per_group(text_ctas)
         self.streams = [torch.cuda.Stream(device=dev) for _ in self.executors]
         self._i = 0
         self.device = dev

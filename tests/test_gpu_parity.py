@@ -177,14 +177,14 @@ def test_forward_device_single_call_matches_compiled_path():
 
 
 @pytest.mark.parametrize('cluster', ['1', '2', '4'])
-def test_tree_cluster_sizes_agree(cluster, monkeypatch):
+def test_tree_cluster_sizes_agree(cluster):
     """The tree kernel gives the same scores whether a question runs on 1, 2 or 4 CTAs."""
     from n2nmn_b200 import weights as wts
-    monkeypatch.setenv('N2NMN_TREE_CLUSTER', cluster)
     N, H, Wd, D, T, C = 24, 10, 15, 512, 20, 28
     feat, word_vecs = synth.make_inputs(N, H, Wd, D, T, seed=41)
     W = wts.init_weights('clevr', H, Wd, D, C, seed=4, bias_std=0.1)
     ex = make_executor('clevr', feat, word_vecs, C, W)
+    ex.set_tree_cluster(int(cluster))
     tokens = synth.expert_mix_tokens(ex.assembler, N, T)
     scores, _ = ex.forward_tokens(tokens)
     ref_s, _, _ = _oracle_scores('clevr', feat, word_vecs, C, W, tokens)

@@ -102,6 +102,17 @@ def test_schedule_accounting_matches_survey_example():
     assert info.num_find_nodes == 2 and info.num_text_nodes == 3
 
 
+def test_contraction_tiles_one_per_layer_and_pass():
+    """num_proj_tiles counts the contraction's 128-row tiles: one per (rows, layer, pass of <= 8
+    fused Find consumers)."""
+    asm = Assembler(synth.vocab_file('clevr'))
+    N = 10   # 10 images x 150 pixels = 12 tiles of 128 rows
+    one = synth.tokens_from_layouts(asm, [['_Find', '_Exist']] * N, 12)
+    assert host_compile('clevr', one)[2].num_proj_tiles == 12
+    nine = synth.tokens_from_layouts(asm, [['_Find'] + ['_Filter'] * 8 + ['_Exist']] * N, 12)
+    assert host_compile('clevr', nine)[2].num_proj_tiles == 24
+
+
 def test_capi_exports_every_declared_symbol():
     """The .so loads and exports exactly what include/n2nmn_b200.h declares (no compute here)."""
     hdr = open(os.path.join(os.path.dirname(GOLDEN), '..', 'include', 'n2nmn_b200.h')).read()

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-launch CUDA-event timing of the three forward kernels when ONE set of launches covers G
 batches (n2nmn_forward_group), G = 1, 2, 4, 8 (GB_ONLY=8: one G only). Env: GB_BATCH, GB_LAYOUT (expert|find), GB_ONLY, GB_ITERS,
-GB_CLUSTER (tree CTAs per question, default 1), GB_TEXT (text CTAs per node group, default 1)."""
+GB_CLUSTER (tree CTAs per question, default 1)."""
 import os, sys
 import numpy as np
 import torch
@@ -28,7 +28,6 @@ for i in range(P):
 ex = LayoutExecutor('clevr', feats[0], wvs[0], C, asm, weights=weights, max_batch=B, max_T=T,
                     max_group=int(os.environ.get('GB_MAXG', 16)))
 ex.set_tree_cluster(int(os.environ.get('GB_CLUSTER', 1)))
-ex.set_text_ctas_per_group(int(os.environ.get('GB_TEXT', 1)))
 only = os.environ.get('GB_ONLY')
 iters = int(os.environ.get('GB_ITERS', 40))
 pk_tf32, pk_hbm = 840.25, 6581.6
@@ -51,7 +50,7 @@ for G in ([int(only)] if only else [1, 2, 4, 8, 16]):
     fl, by = info['kernel_flops'][1], info['kernel_bytes'][1]
     pu = med.get('proj_wgmma_kernel', float('nan'))
     print('G=%d B=%d %s | us per launch (median): %s | per batch: %s | proj: %.1f TF/s = %.3f of TF32 '
-          'peak, %.0f GB/s = %.3f of HBM peak, items %d' % (
+          'peak, %.0f GB/s = %.3f of HBM peak, tiles %d' % (
               G, B, layout, {k: round(v, 1) for k, v in med.items()},
               {k: round(v / G, 2) for k, v in med.items()}, fl / pu / 1e6, fl / pu / 1e6 / pk_tf32,
               by / pu / 1e3, by / pu / 1e3 / pk_hbm, info['num_proj_tiles']), flush=True)

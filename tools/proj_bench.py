@@ -5,10 +5,7 @@ headline shape (64 x 10x15x512, T=20) per set of launches (n2nmn_forward_group),
 events (library profiling mode). Prints the median us per launch of every kernel, the card and its
 power limit.
 
-    python tools/proj_bench.py [--groups 40] [--proj-ctas 0]
-
-With N2NMN_LIB=<experiment build> (tools/build_variants.py attrib) the difference to the default
-library says how much of the kernel is the epilogue, the weight stream and the tensor work."""
+    python tools/proj_bench.py [--groups 40] [--proj-ctas 0]"""
 import argparse, json, os, subprocess, sys
 import numpy as np
 import torch
@@ -61,7 +58,7 @@ try:
 except Exception as e:   # noqa: BLE001
     smi = 'unknown (%s)' % e
 med = {k: round(float(np.median(v)), 1) for k, v in acc.items()}
-print(json.dumps({'lib': os.environ.get('N2NMN_LIB', 'default'), 'card': torch.cuda.get_device_name(),
+print(json.dumps({'card': torch.cuda.get_device_name(),
                   'power_limit_and_max_sm_clock': smi, 'batches_per_launch': G,
                   'proj_ctas': args.proj_ctas, 'groups': args.groups,
                   'proj_wgmma_kernel_us': med.get('proj_wgmma_kernel'), 'median_us': med}))
